@@ -21,10 +21,26 @@ def build_oracle():
     subprocess.check_call(["make", "-s", "-C", HERE, "oracle"])
 
 
+def _is_welle_io(d):
+    return os.path.isfile(os.path.join(d, "src", "backend", "ofdm-processor.cpp")) and os.path.isfile(os.path.join(d, "src", "input", "raw_file.cpp"))
+
+
 def reference_sources():
-    """the welle.io source tree (the directory holding src/) named by $WELLE_IO_SRC, or None"""
+    """the welle.io source tree (the directory holding src/): the one $WELLE_IO_SRC names, else a checkout called `welle.io` or
+    `reference` beside this repository or beside one of the directories above it, else None"""
     d = os.environ.get("WELLE_IO_SRC")
-    return d if d and os.path.isdir(os.path.join(d, "src")) else None
+    if d:
+        return d if os.path.isdir(os.path.join(d, "src")) else None
+    up = os.path.dirname(HERE)
+    while True:
+        parent = os.path.dirname(up)
+        if parent == up:
+            return None
+        for name in ("welle.io", "reference"):
+            cand = os.path.join(parent, name)
+            if cand != up and _is_welle_io(cand):
+                return cand
+        up = parent
 
 
 def build_ref():

@@ -101,7 +101,7 @@ int launch_osc_verify(const DevTables& tb, cudaStream_t st);
 // protection profile -> (L, PI) blocks; returns punctured length or -1
 struct ProtProfile { int bitrate; int nblk; int L[4]; int PI[4]; int in_bits; };
 int make_prot_profile(int bitrate, int short_form, int uep_level, int eep_profile_a, int eep_level, ProtProfile& out);
-// mother-code map: for each of 4*(24*bitrate+6) positions the index into the punctured input or -1
+// mother-code map: for each of 4*(24*bitrate+6) positions the index into the punctured input (saturating at 32767) or -1
 void build_msc_map(const HostTables& t, const ProtProfile& p, int16_t* map);
 
 } // namespace dabb

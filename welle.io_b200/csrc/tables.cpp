@@ -206,10 +206,13 @@ int make_prot_profile(int b, int short_form, int uep_level, int eep_profile_a, i
 
 void build_msc_map(const HostTables& t, const ProtProfile& p, int16_t* map)
 {
+    // build_vit_tables reads only the sign (the softbits are consumed in order), so the index saturates instead of wrapping negative:
+    // EEP 1-A above 341 kbit/s has more than 32767 softbits per codeword
     int pos = 0, ic = 0;
+    auto next = [&ic]() { const int v = ic++; return (int16_t)(v < 32767 ? v : 32767); };
     for (int k = 0; k < p.nblk; k++)
-        for (int i = 0; i < p.L[k] * 128; i++, pos++) map[pos] = t.pcodes[p.PI[k] - 1][i & 31] ? (int16_t)ic++ : (int16_t)-1;
-    for (int i = 0; i < 24; i++, pos++) map[pos] = ((i & 3) < 2) ? (int16_t)ic++ : (int16_t)-1;
+        for (int i = 0; i < p.L[k] * 128; i++, pos++) map[pos] = t.pcodes[p.PI[k] - 1][i & 31] ? next() : (int16_t)-1;
+    for (int i = 0; i < 24; i++, pos++) map[pos] = ((i & 3) < 2) ? next() : (int16_t)-1;
 }
 
 } // namespace dabb
