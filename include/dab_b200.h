@@ -170,6 +170,9 @@ typedef struct {
                                 host->device again.  0 = copy the whole window.  Ignored by dabb_process / dabb_process_async. */
 } dabb_io;
 enum { DABB_IQ_CF32 = 0, DABB_IQ_U8 = 1, DABB_IQ_S8 = 2, DABB_IQ_S16LE = 3, DABB_IQ_S16BE = 4 };
+/* dabb_process and dabb_submit check their arguments before anything is enqueued: a call refused with DABB_E_ARG or DABB_E_STATE
+ * (for example an msc_stride below 3*bitrate or an sf_stride below 15*bitrate of a selected sub-channel) runs no step and leaves
+ * every stream's state as it was. */
 int dabb_process(dabb_ctx* ctx, const dabb_io* io);
 /* asynchronous form for benchmarking with device-resident inputs: enqueue only, no host copies */
 int dabb_process_async(dabb_ctx* ctx, const dabb_io* io);

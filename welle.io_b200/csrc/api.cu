@@ -47,45 +47,82 @@ struct StepScratch {        // per stream, rewritten every step
 
 std::string g_create_error;
 
+// Sole owner of one device or pinned host allocation of n elements, freed when the holder is reallocated, reassigned or destroyed.
+// It converts to T*, so kernels and copies take it where they take a raw pointer.
+template <typename T, bool Pinned> class Owned {
+public:
+    Owned() = default;
+    Owned(const Owned&) = delete;
+    Owned& operator=(const Owned&) = delete;
+    Owned(Owned&& o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+    Owned& operator=(Owned&& o) noexcept { if (this != &o) { reset(); p_ = o.p_; n_ = o.n_; o.p_ = nullptr; o.n_ = 0; } return *this; }
+    ~Owned() { reset(); }
+    // frees the old buffer first; an empty request still gets 16 bytes, so that a successful allocation is never null
+    cudaError_t alloc(size_t n)
+    {
+        reset();
+        void* q = nullptr;
+        const size_t bytes = n * sizeof(T) > 0 ? n * sizeof(T) : 16;
+        const cudaError_t e = Pinned ? cudaHostAlloc(&q, bytes, cudaHostAllocDefault) : cudaMalloc(&q, bytes);
+        if (e == cudaSuccess) { p_ = (T*)q; n_ = n; }
+        return e;
+    }
+    void reset() { if (p_) { if (Pinned) cudaFreeHost(p_); else cudaFree(p_); } p_ = nullptr; n_ = 0; }
+    T* get() const { return p_; }
+    operator T*() const { return p_; }
+    size_t size() const { return n_; }
+private:
+    T* p_ = nullptr;
+    size_t n_ = 0;
+};
+template <typename T> using DevBuf = Owned<T, false>;
+template <typename T> using HostBuf = Owned<T, true>;
+
+// where a step's outputs go in the caller's memory (the output half of dabb_io, or a tap's buffer); any pointer may be null
+struct StepOut {
+    dabb_frame_result* results; uint8_t* fibs; uint8_t* msc; int64_t msc_stride; uint8_t* sf; int64_t sf_stride;
+};
+
 } // namespace
 
 struct dabb_ctx {
     int device = 0; cudaStream_t stream = nullptr; cudaStream_t streamB = nullptr; cudaEvent_t evA[2] = {nullptr, nullptr}, evB[2] = {nullptr, nullptr}; bool evB_valid[2] = {false, false};
-    int64_t step = 0; int last_parity = 0; int32_t* d_fic_ratio = nullptr; int32_t* d_coarse = nullptr; int ofdm_smem_floor = 0; int vit_stages_now = 3;
+    int64_t step = 0; int last_parity = 0; DevBuf<int32_t> d_fic_ratio, d_coarse; int ofdm_smem_floor = 0; int vit_stages_now = 3;
     int prio_b = 0; cudaStream_t streamP = nullptr; cudaEvent_t evPre = nullptr, evPost = nullptr;      // time-sync kernels of lane A at the highest priority (see dabb_create)
-    cudaStream_t stream2 = nullptr; cudaEvent_t ev_ofdm = nullptr, ev_fic = nullptr; uint2* d_dec_fic = nullptr; int S = 0; int fft_mode = 0; int disable_coarse = 0; int keep_taps = 0; int placement = 0; int freqsync = 0;
-    int decode_tii = 0; float2* d_tii = nullptr; bool persistent = false; unsigned int* d_work = nullptr; TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0; int flen_max = 0;
+    cudaStream_t stream2 = nullptr; cudaEvent_t ev_ofdm = nullptr, ev_fic = nullptr; DevBuf<uint2> d_dec_fic; int S = 0; int fft_mode = 0; int disable_coarse = 0; int keep_taps = 0; int placement = 0; int freqsync = 0;
+    int decode_tii = 0; DevBuf<float2> d_tii; bool persistent = false; DevBuf<unsigned int> d_work; TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0; int flen_max = 0;
+    DevBuf<unsigned long long> d_trace_rec; DevBuf<unsigned int> d_trace_count;      // what `trace` points into
     std::string err; int64_t launches = 0; int osc_mismatches = -1; int osc_patched = 0; std::vector<float2> h_osc;
     HostTables* host = nullptr; DevTables dev{};
-    std::vector<void*> allocs;
-    StreamState* d_state = nullptr; StepScratch* d_scr = nullptr; MscSlotState* d_slots = nullptr;
-    int64_t* d_buf_start = nullptr; int64_t* d_win = nullptr; int64_t* d_prs = nullptr; int32_t* d_nco_sync = nullptr; int32_t* d_nco_frame = nullptr;
-    int32_t* d_active = nullptr; int32_t* d_index = nullptr; float* d_cir = nullptr; float* d_cir_work = nullptr; int search_generic = 0; int vit_split = 0; float2* d_r1 = nullptr; float2* d_null = nullptr; int32_t* d_snr = nullptr; float2* d_fc = nullptr; float* d_lvl = nullptr;
-    int8_t* d_soft = nullptr; uint2* d_fic_steptab = nullptr; uint32_t* d_fic_stage_off = nullptr; uint2* d_dec = nullptr; size_t dec_bytes = 0; uint8_t* d_fibs = nullptr; int32_t* d_crc = nullptr;
-    dabb_frame_result* d_results = nullptr;
-    // per slot
+    DevBuf<float2> d_tw_fwd, d_tw_inv, d_prs_ref, d_osc; DevBuf<int16_t> d_invperm, d_fic_map; DevBuf<uint8_t> d_gf_exp, d_gf_log, d_prbs; DevBuf<double2> d_osc_hi;   // what `dev` points into
+    DevBuf<StreamState> d_state; DevBuf<StepScratch> d_scr; DevBuf<MscSlotState> d_slots;
+    DevBuf<int64_t> d_buf_start, d_win, d_prs; DevBuf<int32_t> d_nco_sync, d_nco_frame;
+    DevBuf<int32_t> d_active, d_index; DevBuf<float> d_cir, d_cir_work; int search_generic = 0; int vit_split = 0; DevBuf<float2> d_r1, d_null; DevBuf<int32_t> d_snr; DevBuf<float2> d_fc; DevBuf<float> d_lvl;
+    DevBuf<int8_t> d_soft; DevBuf<uint2> d_fic_steptab; DevBuf<uint32_t> d_fic_stage_off; DevBuf<uint2> d_dec; DevBuf<uint8_t> d_fibs; DevBuf<int32_t> d_crc;
+    DevBuf<dabb_frame_result> d_results;
+    // per slot: everything sized by the slot's code geometry, so that a new geometry starts from an empty Slot
     struct Slot {
-        bool configured = false; ProtProfile prof{}; int nsteps = 0, nbits = 0, frag_pitch = 0, flen = 0;
-        uint2* d_steptab = nullptr; uint32_t* d_stage_off = nullptr; uint32_t* d_prbs_words = nullptr; int8_t* d_frag = nullptr; int32_t* d_valid = nullptr;
-        uint8_t* d_logical = nullptr; uint2* d_dec = nullptr; int8_t* d_ring = nullptr; uint8_t* d_window = nullptr; uint8_t* d_sf = nullptr; int32_t* d_info = nullptr;
+        bool configured = false; ProtProfile prof{}; int nsteps = 0, nbits = 0, frag_pitch = 0, flen = 0, flen_pad = 0;
+        DevBuf<uint2> d_steptab; DevBuf<uint32_t> d_stage_off, d_prbs_words; DevBuf<int8_t> d_frag; DevBuf<int32_t> d_valid;
+        DevBuf<uint8_t> d_logical; DevBuf<uint2> d_dec; DevBuf<uint8_t> d_window, d_sf; DevBuf<int32_t> d_info;
     } slot[DABB_MAX_SUBCH];
-    uint32_t* d_fic_prbs_words = nullptr;
+    DevBuf<int8_t> d_ring[DABB_MAX_SUBCH];     // per slot: the time de-interleaver's history, kept when the slot's geometry changes
+    DevBuf<uint32_t> d_fic_prbs_words;
     std::vector<MscSlotState> h_slots;
-    float2* d_iq_stage = nullptr; size_t iq_stage_samples = 0; uint8_t* d_raw_stage = nullptr; size_t raw_stage_bytes = 0;
+    DevBuf<float2> d_iq_stage; DevBuf<uint8_t> d_raw_stage;
     // pipelined host-buffer path (dabb_submit / dabb_collect): copy stream, two device staging slots, two result slots in pinned memory
     cudaStream_t streamC = nullptr; cudaEvent_t evH2D[2] = {nullptr, nullptr}, evStageFree[2] = {nullptr, nullptr}; bool stageFreeValid[2] = {false, false};
-    void* d_stage2[2] = {nullptr, nullptr}; size_t stage2_bytes[2] = {0, 0};
+    DevBuf<uint8_t> d_stage2[2];
     int stage_last_fmt = -1; int64_t stage_last_len = 0; std::vector<int64_t> stage_last_start;     // the previous dabb_submit's window (carry_samples)
+    // one step's outputs on their way to the caller: device -> pinned copies, complete at `done`, then scattered into `out`
     struct Pending {
-        bool used = false; cudaEvent_t done = nullptr; dabb_io io{};
-        dabb_frame_result* h_res = nullptr; uint8_t* h_fibs = nullptr; uint8_t* h_msc = nullptr; uint8_t* h_sf = nullptr; size_t msc_bytes = 0, sf_bytes = 0;
-        int flen[DABB_MAX_SUBCH] = {0, 0, 0, 0}; size_t msc_off[DABB_MAX_SUBCH] = {0, 0, 0, 0}, sf_off[DABB_MAX_SUBCH] = {0, 0, 0, 0};
-    } pend[2];
+        cudaEvent_t done = nullptr; StepOut out{};
+        HostBuf<dabb_frame_result> h_res; HostBuf<uint8_t> h_fibs, h_logical, h_superframe;
+        int flen[DABB_MAX_SUBCH] = {0, 0, 0, 0}, flen_pad[DABB_MAX_SUBCH] = {0, 0, 0, 0}; size_t msc_off[DABB_MAX_SUBCH] = {0, 0, 0, 0}, sf_off[DABB_MAX_SUBCH] = {0, 0, 0, 0};
+    } pend[2], pend_sync;     // the two dabb_submit slots; dabb_process and taps 7 / 8, which never leave a step outstanding
     int pend_head = 0, pend_count = 0; int64_t submits = 0;
-    // pinned host staging for results
-    dabb_frame_result* h_results = nullptr; uint8_t* h_fibs = nullptr; uint8_t* h_msc = nullptr; uint8_t* h_sf = nullptr;
     int groups = 1; int fc_pitch = 1; int tail_frames = 0; int tail_groups = 5; int nco_fast = 0;
-    const int32_t** d_info_tab = nullptr;
+    DevBuf<const int32_t*> d_info_tab;
     // optional per-kernel timing: one event after every launch, durations = differences of consecutive events
     bool prof = false; std::vector<cudaEvent_t> prof_ev; std::vector<const char*> prof_name; size_t prof_used = 0;
     std::vector<std::pair<std::string, std::pair<double, long>>> prof_acc;
@@ -95,24 +132,20 @@ namespace {
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_); return DABB_E_CUDA; } } while (0)
 
-template <typename T> int dalloc(dabb_ctx* ctx, T** p, size_t n, bool zero = true)
+template <typename T, bool Pinned> int alloc(dabb_ctx* ctx, Owned<T, Pinned>& b, size_t n)
 {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, n * sizeof(T) > 0 ? n * sizeof(T) : 16);
-    if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc: ") + cudaGetErrorString(e); return DABB_E_NOMEM; }
-    if (zero) cudaMemsetAsync(q, 0, n * sizeof(T), ctx->stream);
-    ctx->allocs.push_back(q);
-    *p = (T*)q;
-    return 0;
+    const cudaError_t e = b.alloc(n);
+    if (e == cudaSuccess) return 0;
+    ctx->err = std::string(Pinned ? "pinned host" : "device") + " allocation of " + std::to_string(n * sizeof(T)) + " bytes failed: " + cudaGetErrorString(e);
+    return DABB_E_NOMEM;
 }
 
-// frees a device allocation made through dalloc / tracked in ctx->allocs
-template <typename T> void dfree(dabb_ctx* ctx, T*& p)
+// a device buffer, zero-filled on the context's stream unless `zero` is false
+template <typename T> int dalloc(dabb_ctx* ctx, DevBuf<T>& b, size_t n, bool zero = true)
 {
-    if (!p) return;
-    for (size_t i = 0; i < ctx->allocs.size(); i++) if (ctx->allocs[i] == (void*)p) { ctx->allocs.erase(ctx->allocs.begin() + i); break; }
-    cudaFree((void*)p);
-    p = nullptr;
+    const int rc = alloc(ctx, b, n);
+    if (!rc && zero) cudaMemsetAsync(b.get(), 0, n * sizeof(T), ctx->stream);
+    return rc;
 }
 
 void prof_mark(dabb_ctx* ctx, const char* what)
@@ -402,6 +435,7 @@ void sync_all(dabb_ctx* ctx)
     if (ctx->streamP) cudaStreamSynchronize(ctx->streamP);
     if (ctx->streamB) cudaStreamSynchronize(ctx->streamB);
     if (ctx->stream2) cudaStreamSynchronize(ctx->stream2);
+    if (ctx->streamC) cudaStreamSynchronize(ctx->streamC);
 }
 
 // raw file formats -> cf32, value for value like CRAWFile::convertSamples (input/raw_file.cpp:336-363): u8 (b-128)/128,
@@ -424,16 +458,91 @@ __global__ void convert_iq_kernel(const uint8_t* __restrict__ raw, int64_t raw_s
     out[(int64_t)s * out_stride + i] = make_float2(re, im);
 }
 
-int ensure_dec(dabb_ctx* ctx, size_t bytes)
+// makes b hold at least n elements, without keeping its contents; the device finishes with the old buffer first
+template <typename T> int grow(dabb_ctx* ctx, DevBuf<T>& b, size_t n)
 {
-    if (bytes <= ctx->dec_bytes) return 0;
-    if (ctx->d_dec) { cudaStreamSynchronize(ctx->stream); dfree(ctx, ctx->d_dec); ctx->dec_bytes = 0; }
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, bytes);
-    if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc(decisions): ") + cudaGetErrorString(e); return DABB_E_NOMEM; }
-    ctx->allocs.push_back(q);
-    ctx->d_dec = (uint2*)q; ctx->dec_bytes = bytes;
-    return 0;
+    if (n <= b.size()) return 0;
+    sync_all(ctx);
+    return alloc(ctx, b, n);
+}
+
+size_t bytes_per_sample(int fmt) { return fmt == DABB_IQ_CF32 ? 8 : ((fmt == DABB_IQ_U8 || fmt == DABB_IQ_S8) ? 2 : 4); }
+
+// ---- step outputs ---------------------------------------------------------------------------------------------------------------
+// Every way a step's outputs reach the caller (dabb_process, dabb_submit + dabb_collect, taps 7 / 8) runs the same three routines:
+// prepare_pending sizes a Pending's pinned buffers for the configured slots, enqueue_readback copies the device buffers whole into it
+// behind the step, and deliver writes them into the caller's layout [S][MAX_SUBCH][4][msc_stride] / [S][MAX_SUBCH][sf_stride].
+// check_strides runs before any of them and before the step, so that a refused call has enqueued nothing.
+
+StepOut step_out(const dabb_io& io) { return StepOut{io.results, io.fibs, io.msc, io.msc_stride, io.sf, io.sf_stride}; }
+
+int check_strides(dabb_ctx* ctx, const StepOut& o)
+{
+    for (int k = 0; k < ctx->n_slots; k++) {
+        const auto& sl = ctx->slot[k];
+        if (!sl.configured) continue;
+        if (o.msc && o.msc_stride < sl.flen) { ctx->err = "msc_stride smaller than the logical frame"; return DABB_E_ARG; }
+        if (o.sf && o.sf_stride < 5 * sl.flen) { ctx->err = "sf_stride smaller than the superframe"; return DABB_E_ARG; }
+    }
+    return DABB_OK;
+}
+
+// p must not have copies in flight (collected, or never used)
+int prepare_pending(dabb_ctx* ctx, dabb_ctx::Pending& p)
+{
+    const int S = ctx->S;
+    int rc;
+    if (!p.done) CK(cudaEventCreateWithFlags(&p.done, cudaEventDisableTiming));
+    if (!p.h_res && (rc = alloc(ctx, p.h_res, S))) return rc;
+    if (!p.h_fibs && (rc = alloc(ctx, p.h_fibs, (size_t)S * 12 * 32))) return rc;
+    size_t msc = 0, sf = 0;
+    for (int k = 0; k < ctx->n_slots; k++) {
+        const auto& sl = ctx->slot[k];
+        p.flen[k] = sl.configured ? sl.flen : 0; p.flen_pad[k] = sl.flen_pad;
+        if (!sl.configured) continue;
+        p.msc_off[k] = msc; p.sf_off[k] = sf;
+        msc += (size_t)S * 4 * sl.flen_pad; sf += (size_t)S * 5 * sl.flen_pad;
+    }
+    if (msc > p.h_logical.size() && (rc = alloc(ctx, p.h_logical, msc))) return rc;
+    if (sf > p.h_superframe.size() && (rc = alloc(ctx, p.h_superframe, sf))) return rc;
+    return DABB_OK;
+}
+
+// the outputs `o` asks for, device -> p, on lane B (the main stream while profiling) behind the last step's result record
+int enqueue_readback(dabb_ctx* ctx, dabb_ctx::Pending& p, const StepOut& o)
+{
+    const int S = ctx->S;
+    cudaStream_t B = ctx->prof ? ctx->stream : ctx->streamB;
+    if (o.results) CK(cudaMemcpyAsync(p.h_res, ctx->d_results, sizeof(dabb_frame_result) * S, cudaMemcpyDeviceToHost, B));
+    if (o.fibs) CK(cudaMemcpyAsync(p.h_fibs, ctx->d_fibs, (size_t)S * 12 * 32, cudaMemcpyDeviceToHost, B));
+    for (int k = 0; k < ctx->n_slots; k++) {
+        if (!p.flen[k]) continue;
+        const auto& sl = ctx->slot[k];
+        if (o.msc) CK(cudaMemcpyAsync(p.h_logical + p.msc_off[k], sl.d_logical, (size_t)S * 4 * p.flen_pad[k], cudaMemcpyDeviceToHost, B));
+        if (o.sf) CK(cudaMemcpyAsync(p.h_superframe + p.sf_off[k], sl.d_sf, (size_t)S * 5 * p.flen_pad[k], cudaMemcpyDeviceToHost, B));
+    }
+    CK(cudaEventRecord(p.done, B));
+    p.out = o;
+    return DABB_OK;
+}
+
+int deliver(dabb_ctx* ctx, dabb_ctx::Pending& p)
+{
+    CK(cudaEventSynchronize(p.done));
+    const int S = ctx->S;
+    const StepOut& o = p.out;
+    if (o.results) memcpy(o.results, p.h_res, sizeof(dabb_frame_result) * S);
+    if (o.fibs) memcpy(o.fibs, p.h_fibs, (size_t)S * 12 * 32);
+    for (int k = 0; k < ctx->n_slots; k++) {
+        const size_t flen = p.flen[k], fp = p.flen_pad[k];
+        if (!flen) continue;
+        if (o.msc)       // pinned rows [S*4][fp] -> caller [S][MAX_SUBCH][4][msc_stride]
+            for (int s = 0; s < S; s++) for (int c = 0; c < 4; c++)
+                memcpy(o.msc + (((size_t)s * DABB_MAX_SUBCH + k) * 4 + c) * o.msc_stride, p.h_logical + p.msc_off[k] + ((size_t)s * 4 + c) * fp, flen);
+        if (o.sf)
+            for (int s = 0; s < S; s++) memcpy(o.sf + ((size_t)s * DABB_MAX_SUBCH + k) * o.sf_stride, p.h_superframe + p.sf_off[k] + (size_t)s * 5 * fp, 5 * flen);
+    }
+    return DABB_OK;
 }
 
 } // namespace
@@ -510,9 +619,10 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     if (getenv("DABB_TAIL_GROUPS")) { const int v = atoi(getenv("DABB_TAIL_GROUPS")); if (v > 0 && 75 % v == 0) ctx->tail_groups = v; }
     ctx->fc_pitch = ctx->tail_frames ? ctx->tail_groups : ctx->groups;
     // tables
-    float2 *tf, *ti, *pr, *osc; int16_t *ip, *fm; uint8_t *ge, *gl, *pb;
-    if ((rc = dalloc(ctx, &tf, TwLayout::TOTAL)) || (rc = dalloc(ctx, &ti, TwLayout::TOTAL)) || (rc = dalloc(ctx, &pr, TU)) || (rc = dalloc(ctx, &osc, INPUT_RATE, false)) ||
-        (rc = dalloc(ctx, &ip, sizeof ctx->host->invperm / sizeof(int16_t))) || (rc = dalloc(ctx, &fm, 3096)) || (rc = dalloc(ctx, &ge, 512)) || (rc = dalloc(ctx, &gl, 256)) || (rc = dalloc(ctx, &pb, sizeof ctx->host->prbs)))
+    auto& tf = ctx->d_tw_fwd; auto& ti = ctx->d_tw_inv; auto& pr = ctx->d_prs_ref; auto& osc = ctx->d_osc; auto& ip = ctx->d_invperm; auto& fm = ctx->d_fic_map;
+    auto& ge = ctx->d_gf_exp; auto& gl = ctx->d_gf_log; auto& pb = ctx->d_prbs;
+    if ((rc = dalloc(ctx, tf, TwLayout::TOTAL)) || (rc = dalloc(ctx, ti, TwLayout::TOTAL)) || (rc = dalloc(ctx, pr, TU)) || (rc = dalloc(ctx, osc, INPUT_RATE, false)) ||
+        (rc = dalloc(ctx, ip, sizeof ctx->host->invperm / sizeof(int16_t))) || (rc = dalloc(ctx, fm, 3096)) || (rc = dalloc(ctx, ge, 512)) || (rc = dalloc(ctx, gl, 256)) || (rc = dalloc(ctx, pb, sizeof ctx->host->prbs)))
         return fail(rc);
     {
         ctx->h_osc.resize(INPUT_RATE);
@@ -533,8 +643,8 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     {
         // on-the-fly oscillator: upload the factors, compare against the table for every index on the device, adopt it only when
         // nothing differs; DABB_OSC_TABLE=1 in the environment forces the table lookups (A/B measurements)
-        double2* hi;
-        if ((rc = dalloc(ctx, &hi, 2000))) return fail(rc);
+        auto& hi = ctx->d_osc_hi;
+        if ((rc = dalloc(ctx, hi, 2000))) return fail(rc);
         std::vector<double2> h_hi(2000);
         build_osc_factors(ctx->h_osc.data(), h_hi.data(), &ctx->dev.osc_theta, &ctx->osc_patched);
         cudaMemcpyAsync(hi, h_hi.data(), sizeof(double2) * 2000, cudaMemcpyHostToDevice, ctx->stream);
@@ -546,12 +656,12 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     }
     {
         std::vector<uint32_t> w; pack_prbs_words(ctx->host->prbs, 768, w);
-        if ((rc = dalloc(ctx, &ctx->d_fic_prbs_words, w.size()))) return fail(rc);
+        if ((rc = dalloc(ctx, ctx->d_fic_prbs_words, w.size()))) return fail(rc);
         cudaMemcpy(ctx->d_fic_prbs_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice);
         // expansion tables of the decoder kernel for the FIC puncturing (fic-handler.cpp:144-191)
         std::vector<uint2> steps; std::vector<uint32_t> soff;
         build_vit_tables_u2(ctx->host->fic_map, 774, steps, soff);
-        if ((rc = dalloc(ctx, &ctx->d_fic_steptab, steps.size())) || (rc = dalloc(ctx, &ctx->d_fic_stage_off, soff.size()))) return fail(rc);
+        if ((rc = dalloc(ctx, ctx->d_fic_steptab, steps.size())) || (rc = dalloc(ctx, ctx->d_fic_stage_off, soff.size()))) return fail(rc);
         cudaMemcpy(ctx->d_fic_steptab, steps.data(), steps.size() * sizeof(uint2), cudaMemcpyHostToDevice);
         cudaMemcpy(ctx->d_fic_stage_off, soff.data(), soff.size() * 4, cudaMemcpyHostToDevice);
     }
@@ -559,24 +669,23 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     ctx->search_generic = getenv("DABB_SEARCH_GENERIC") != nullptr;     // A/B: ThresholdBeforePeak through the literal sliding maximum
     if (getenv("DABB_TRACE")) {
         ctx->trace_path = getenv("DABB_TRACE"); ctx->trace.cap = 1u << 20;
-        if ((rc = dalloc(ctx, &ctx->trace.rec, (size_t)3 * ctx->trace.cap)) || (rc = dalloc(ctx, &ctx->trace.count, 1))) return fail(rc);
+        if ((rc = dalloc(ctx, ctx->d_trace_rec, (size_t)3 * ctx->trace.cap)) || (rc = dalloc(ctx, ctx->d_trace_count, 1))) return fail(rc);
+        ctx->trace.rec = ctx->d_trace_rec; ctx->trace.count = ctx->d_trace_count;
     }
     ctx->ring_pitch = ctx->max_cu * 64;
-    if ((rc = dalloc(ctx, &ctx->d_state, S)) || (rc = dalloc(ctx, &ctx->d_scr, 2 * (size_t)S)) || (rc = dalloc(ctx, &ctx->d_fic_ratio, S)) || (rc = dalloc(ctx, &ctx->d_coarse, S)) || (rc = dalloc(ctx, &ctx->d_slots, (size_t)S * ctx->n_slots)) ||
-        (rc = dalloc(ctx, &ctx->d_buf_start, S)) || (rc = dalloc(ctx, &ctx->d_win, 2 * (size_t)S)) || (rc = dalloc(ctx, &ctx->d_prs, 2 * (size_t)S)) ||
-        (rc = dalloc(ctx, &ctx->d_nco_sync, 4 * (size_t)S)) || (rc = dalloc(ctx, &ctx->d_nco_frame, 8 * (size_t)S)) || (rc = dalloc(ctx, &ctx->d_active, 2 * (size_t)S)) ||
-        (rc = dalloc(ctx, &ctx->d_index, 2 * (size_t)S)) || (rc = dalloc(ctx, &ctx->d_snr, 2 * (size_t)S)) || (rc = dalloc(ctx, &ctx->d_fc, 2 * (size_t)S * ctx->fc_pitch)) || (rc = dalloc(ctx, &ctx->d_lvl, 2 * (size_t)S * ctx->fc_pitch)) ||
-        (rc = dalloc(ctx, &ctx->d_soft, 2 * (size_t)S * DABB_SOFT_PER_FRAME + VIT_FRAG_SLACK, false)) ||
-        (rc = dalloc(ctx, &ctx->d_fibs, (size_t)S * 12 * 32)) || (rc = dalloc(ctx, &ctx->d_crc, S)) || (rc = dalloc(ctx, &ctx->d_results, S)) ||
-        (rc = dalloc(ctx, &ctx->d_info_tab, DABB_MAX_SUBCH)) || (rc = dalloc(ctx, &ctx->d_cir_work, (size_t)S * TU, false)))
+    if ((rc = dalloc(ctx, ctx->d_state, S)) || (rc = dalloc(ctx, ctx->d_scr, 2 * (size_t)S)) || (rc = dalloc(ctx, ctx->d_fic_ratio, S)) || (rc = dalloc(ctx, ctx->d_coarse, S)) || (rc = dalloc(ctx, ctx->d_slots, (size_t)S * ctx->n_slots)) ||
+        (rc = dalloc(ctx, ctx->d_buf_start, S)) || (rc = dalloc(ctx, ctx->d_win, 2 * (size_t)S)) || (rc = dalloc(ctx, ctx->d_prs, 2 * (size_t)S)) ||
+        (rc = dalloc(ctx, ctx->d_nco_sync, 4 * (size_t)S)) || (rc = dalloc(ctx, ctx->d_nco_frame, 8 * (size_t)S)) || (rc = dalloc(ctx, ctx->d_active, 2 * (size_t)S)) ||
+        (rc = dalloc(ctx, ctx->d_index, 2 * (size_t)S)) || (rc = dalloc(ctx, ctx->d_snr, 2 * (size_t)S)) || (rc = dalloc(ctx, ctx->d_fc, 2 * (size_t)S * ctx->fc_pitch)) || (rc = dalloc(ctx, ctx->d_lvl, 2 * (size_t)S * ctx->fc_pitch)) ||
+        (rc = dalloc(ctx, ctx->d_soft, 2 * (size_t)S * DABB_SOFT_PER_FRAME + VIT_FRAG_SLACK, false)) ||
+        (rc = dalloc(ctx, ctx->d_fibs, (size_t)S * 12 * 32)) || (rc = dalloc(ctx, ctx->d_crc, S)) || (rc = dalloc(ctx, ctx->d_results, S)) ||
+        (rc = dalloc(ctx, ctx->d_info_tab, DABB_MAX_SUBCH)) || (rc = dalloc(ctx, ctx->d_cir_work, (size_t)S * TU, false)))
         return fail(rc);
-    if (ctx->keep_taps && ((rc = dalloc(ctx, &ctx->d_cir, (size_t)S * TU)) || (rc = dalloc(ctx, &ctx->d_r1, (size_t)S * 75 * 1536)) || (rc = dalloc(ctx, &ctx->d_null, (size_t)S * TNULL)))) return fail(rc);
-    if ((rc = ensure_dec(ctx, vit_dec_bytes(S * 4, 774)))) return fail(rc);
-    { void* q = nullptr; if (cudaMalloc(&q, vit_dec_bytes(S * 4, 774)) != cudaSuccess) { ctx->err = "cudaMalloc(FIC decisions)"; return fail(DABB_E_NOMEM); } ctx->allocs.push_back(q); ctx->d_dec_fic = (uint2*)q; }
+    if (ctx->keep_taps && ((rc = dalloc(ctx, ctx->d_cir, (size_t)S * TU)) || (rc = dalloc(ctx, ctx->d_r1, (size_t)S * 75 * 1536)) || (rc = dalloc(ctx, ctx->d_null, (size_t)S * TNULL)))) return fail(rc);
+    if ((rc = dalloc(ctx, ctx->d_dec, vit_dec_bytes(S * 4, 774) / sizeof(uint2), false)) || (rc = dalloc(ctx, ctx->d_dec_fic, vit_dec_bytes(S * 4, 774) / sizeof(uint2), false))) return fail(rc);
     ctx->h_slots.assign((size_t)S * ctx->n_slots, MscSlotState{});
     // info arrays of unconfigured slots are never read (finalize skips disabled slots)
-    cudaHostAlloc((void**)&ctx->h_results, sizeof(dabb_frame_result) * S, cudaHostAllocDefault);
-    cudaHostAlloc((void**)&ctx->h_fibs, (size_t)S * 12 * 32, cudaHostAllocDefault);
+    if ((rc = prepare_pending(ctx, ctx->pend_sync))) return fail(rc);
     {
         reset_kernel<<<(S + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_state, ctx->d_slots, ctx->n_slots, 0, S, 0, ctx->d_fic_ratio);
         ctx->launches++;
@@ -598,23 +707,14 @@ void dabb_destroy(dabb_ctx* ctx)
         cudaMemcpy(h.data(), ctx->trace.rec, h.size() * 8, cudaMemcpyDeviceToHost);
         if (FILE* f = fopen(ctx->trace_path.c_str(), "w")) { for (unsigned int i = 0; i < n; i++) fprintf(f, "%llu %llu %llu %llu\n", h[3 * i] >> 32, h[3 * i] & 0xFFFFFFFFull, h[3 * i + 1], h[3 * i + 2]); fclose(f); }
     }
-    for (void* p : ctx->allocs) cudaFree(p);
     for (cudaEvent_t e : ctx->prof_ev) cudaEventDestroy(e);
-    if (ctx->d_iq_stage) cudaFree(ctx->d_iq_stage);
-    if (ctx->d_raw_stage) cudaFree(ctx->d_raw_stage);
     for (int i = 0; i < 2; i++) {
-        if (ctx->d_stage2[i]) cudaFree(ctx->d_stage2[i]);
         if (ctx->evH2D[i]) cudaEventDestroy(ctx->evH2D[i]);
         if (ctx->evStageFree[i]) cudaEventDestroy(ctx->evStageFree[i]);
-        auto& p = ctx->pend[i];
-        if (p.done) cudaEventDestroy(p.done);
-        if (p.h_res) cudaFreeHost(p.h_res); if (p.h_fibs) cudaFreeHost(p.h_fibs); if (p.h_msc) cudaFreeHost(p.h_msc); if (p.h_sf) cudaFreeHost(p.h_sf);
+        if (ctx->pend[i].done) cudaEventDestroy(ctx->pend[i].done);
     }
+    if (ctx->pend_sync.done) cudaEventDestroy(ctx->pend_sync.done);
     if (ctx->streamC) cudaStreamDestroy(ctx->streamC);
-    if (ctx->h_results) cudaFreeHost(ctx->h_results);
-    if (ctx->h_fibs) cudaFreeHost(ctx->h_fibs);
-    if (ctx->h_msc) cudaFreeHost(ctx->h_msc);
-    if (ctx->h_sf) cudaFreeHost(ctx->h_sf);
     if (ctx->ev_ofdm) cudaEventDestroy(ctx->ev_ofdm);
     if (ctx->ev_fic) cudaEventDestroy(ctx->ev_fic);
     for (int i = 0; i < 2; i++) { if (ctx->evA[i]) cudaEventDestroy(ctx->evA[i]); if (ctx->evB[i]) cudaEventDestroy(ctx->evB[i]); }
@@ -625,7 +725,7 @@ void dabb_destroy(dabb_ctx* ctx)
     if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx->host;
-    delete ctx;
+    delete ctx;         // frees every device and pinned buffer
 }
 
 void* dabb_cuda_stream(dabb_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
@@ -671,30 +771,26 @@ int dabb_select_subchannel(dabb_ctx* ctx, int32_t first, int32_t count, int32_t 
         for (int i = 0; i < S; i++) if ((i < first || i >= first + count) && ctx->h_slots[(size_t)i * ctx->n_slots + slot].enabled) others = true;
         if (others) { ctx->err = "streams sharing a slot must use the same bitrate/protection; use another slot"; return DABB_E_UNSUPPORTED; }
         // the slot changes its code geometry: give back the buffers sized for the old one (all streams are idle: sync_all above)
-        dfree(ctx, sl.d_steptab); dfree(ctx, sl.d_stage_off); dfree(ctx, sl.d_prbs_words); dfree(ctx, sl.d_frag); dfree(ctx, sl.d_valid);
-        dfree(ctx, sl.d_logical); dfree(ctx, sl.d_window); dfree(ctx, sl.d_sf); dfree(ctx, sl.d_info); dfree(ctx, sl.d_dec);
-        sl.configured = false;
+        sl = dabb_ctx::Slot{};
     }
     if (!sl.configured) {
-        sl.prof = prof; sl.nbits = 24 * prof.bitrate; sl.nsteps = sl.nbits + 6; sl.frag_pitch = ctx->ring_pitch; sl.flen = 3 * prof.bitrate;
+        sl.prof = prof; sl.nbits = 24 * prof.bitrate; sl.nsteps = sl.nbits + 6; sl.frag_pitch = ctx->ring_pitch; sl.flen = 3 * prof.bitrate; sl.flen_pad = (sl.flen + 15) & ~15;
         std::vector<int16_t> map((size_t)sl.nsteps * 4);
         build_msc_map(*ctx->host, prof, map.data());
         std::vector<uint2> steps; std::vector<uint32_t> soff;
         build_vit_tables_u2(map.data(), sl.nsteps, steps, soff);
         std::vector<uint32_t> w; pack_prbs_words(ctx->host->prbs, sl.nbits, w);
-        const int flen_pad = (sl.flen + 15) & ~15;
-        if ((rc = dalloc(ctx, &sl.d_steptab, steps.size())) || (rc = dalloc(ctx, &sl.d_stage_off, soff.size())) || (rc = dalloc(ctx, &sl.d_prbs_words, w.size())) ||
-            (rc = dalloc(ctx, &sl.d_frag, (size_t)S * 4 * sl.frag_pitch + VIT_FRAG_SLACK)) ||
-            (rc = dalloc(ctx, &sl.d_valid, (size_t)S * 4)) || (rc = dalloc(ctx, &sl.d_logical, (size_t)S * 4 * flen_pad)) ||
-            (rc = dalloc(ctx, &sl.d_window, (size_t)S * 5 * flen_pad)) || (rc = dalloc(ctx, &sl.d_sf, (size_t)S * 5 * flen_pad)) ||
-            (rc = dalloc(ctx, &sl.d_info, (size_t)S * 16)))
+        if ((rc = dalloc(ctx, sl.d_steptab, steps.size())) || (rc = dalloc(ctx, sl.d_stage_off, soff.size())) || (rc = dalloc(ctx, sl.d_prbs_words, w.size())) ||
+            (rc = dalloc(ctx, sl.d_frag, (size_t)S * 4 * sl.frag_pitch + VIT_FRAG_SLACK)) ||
+            (rc = dalloc(ctx, sl.d_valid, (size_t)S * 4)) || (rc = dalloc(ctx, sl.d_logical, (size_t)S * 4 * sl.flen_pad)) ||
+            (rc = dalloc(ctx, sl.d_window, (size_t)S * 5 * sl.flen_pad)) || (rc = dalloc(ctx, sl.d_sf, (size_t)S * 5 * sl.flen_pad)) ||
+            (rc = dalloc(ctx, sl.d_info, (size_t)S * 16)) || (rc = dalloc(ctx, sl.d_dec, vit_dec_bytes(S * 4, sl.nsteps) / sizeof(uint2), false)))
             return rc;
-        if (!sl.d_ring && (rc = dalloc(ctx, &sl.d_ring, (size_t)S * MSC_RING * ctx->ring_pitch))) return rc;
+        if (!ctx->d_ring[slot] && (rc = dalloc(ctx, ctx->d_ring[slot], (size_t)S * MSC_RING * ctx->ring_pitch))) return rc;
         CK(cudaMemcpyAsync(sl.d_steptab, steps.data(), steps.size() * sizeof(uint2), cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaMemcpyAsync(sl.d_stage_off, soff.data(), soff.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaMemcpyAsync(sl.d_prbs_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        { void* q = nullptr; if (cudaMalloc(&q, vit_dec_bytes(S * 4, sl.nsteps)) != cudaSuccess) { ctx->err = "cudaMalloc(slot decisions)"; return DABB_E_NOMEM; } ctx->allocs.push_back(q); sl.d_dec = (uint2*)q; }
         sl.configured = true;
         if (sl.flen > ctx->flen_max) ctx->flen_max = sl.flen;
     }
@@ -734,6 +830,17 @@ static int run_fic(dabb_ctx* ctx, const int8_t* soft, int64_t soft_stride, const
 
 static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int64_t stride);
 
+// cf32 samples in d_iq_stage from raw-format samples on the device (stream s at raw + s * raw_stride samples), converted on lane A
+static int convert_to_stage(dabb_ctx* ctx, const uint8_t* raw, int64_t raw_stride, int fmt, int64_t len)
+{
+    const int S = ctx->S;
+    int rc;
+    if ((rc = grow(ctx, ctx->d_iq_stage, (size_t)S * len))) return rc;
+    const dim3 grid((unsigned)((len + 255) / 256), (unsigned)S);
+    convert_iq_kernel<<<grid, 256, 0, ctx->stream>>>(raw, raw_stride, fmt, ctx->d_iq_stage, len, len, S);
+    return check_launch(ctx, "convert_iq_kernel");
+}
+
 int dabb_process_async(dabb_ctx* ctx, const dabb_io* io)
 {
     if (!ctx || !io || !io->iq || !io->buf_start) return DABB_E_ARG;
@@ -746,37 +853,19 @@ int dabb_process_async(dabb_ctx* ctx, const dabb_io* io)
     const int fmt = io->iq_format;
     if (fmt < 0 || fmt > DABB_IQ_S16BE) { ctx->err = "unknown iq_format"; return DABB_E_ARG; }
     if (io->iq_is_host || fmt != DABB_IQ_CF32) {
-        const size_t need = (size_t)S * io->buf_len;
-        if (need > ctx->iq_stage_samples) {
-            sync_all(ctx);
-            if (ctx->d_iq_stage) cudaFree(ctx->d_iq_stage);
-            ctx->d_iq_stage = nullptr; ctx->iq_stage_samples = 0;
-            cudaError_t e = cudaMalloc((void**)&ctx->d_iq_stage, need * sizeof(float2));
-            if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc(iq staging): ") + cudaGetErrorString(e); return DABB_E_NOMEM; }
-            ctx->iq_stage_samples = need;
-        }
+        const size_t need = (size_t)S * io->buf_len, bps = bytes_per_sample(fmt);
         if (fmt == DABB_IQ_CF32) {
-            CK(cudaMemcpy2DAsync(ctx->d_iq_stage, (size_t)io->buf_len * sizeof(float2), io->iq, (size_t)stride * sizeof(float2), (size_t)io->buf_len * sizeof(float2), S,
-                                 cudaMemcpyHostToDevice, A));
+            if ((rc = grow(ctx, ctx->d_iq_stage, need))) return rc;
+            CK(cudaMemcpy2DAsync(ctx->d_iq_stage, (size_t)io->buf_len * bps, io->iq, (size_t)stride * bps, (size_t)io->buf_len * bps, S, cudaMemcpyHostToDevice, A));
         } else {
-            const size_t bps = (fmt == DABB_IQ_U8 || fmt == DABB_IQ_S8) ? 2 : 4;
             const uint8_t* raw = reinterpret_cast<const uint8_t*>(io->iq);
             int64_t raw_stride = stride;
             if (io->iq_is_host) {
-                if (need * bps > ctx->raw_stage_bytes) {
-                    sync_all(ctx);
-                    if (ctx->d_raw_stage) cudaFree(ctx->d_raw_stage);
-                    ctx->d_raw_stage = nullptr; ctx->raw_stage_bytes = 0;
-                    cudaError_t e = cudaMalloc((void**)&ctx->d_raw_stage, need * bps);
-                    if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc(raw staging): ") + cudaGetErrorString(e); return DABB_E_NOMEM; }
-                    ctx->raw_stage_bytes = need * bps;
-                }
+                if ((rc = grow(ctx, ctx->d_raw_stage, need * bps))) return rc;
                 CK(cudaMemcpy2DAsync(ctx->d_raw_stage, (size_t)io->buf_len * bps, io->iq, (size_t)stride * bps, (size_t)io->buf_len * bps, S, cudaMemcpyHostToDevice, A));
                 raw = ctx->d_raw_stage; raw_stride = io->buf_len;
             }
-            const dim3 grid((unsigned)((io->buf_len + 255) / 256), (unsigned)S);
-            convert_iq_kernel<<<grid, 256, 0, A>>>(raw, raw_stride, fmt, ctx->d_iq_stage, io->buf_len, io->buf_len, S);
-            if ((rc = check_launch(ctx, "convert_iq_kernel"))) return rc;
+            if ((rc = convert_to_stage(ctx, raw, raw_stride, fmt, io->buf_len))) return rc;
         }
         iq = ctx->d_iq_stage; stride = io->buf_len;
     }
@@ -819,7 +908,7 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     plan_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, ctx->d_buf_start, io->buf_len, S, d_win, d_nco_sync, d_active);
     if ((rc = check_launch(ctx, "plan_kernel"))) return rc;
     SyncParams sp{}; sp.iq = iq; sp.stride = stride; sp.win_start = d_win; sp.nco = d_nco_sync; sp.active = d_active; sp.index_out = d_index; sp.cir_out = ctx->d_cir; sp.n = S;
-    sp.fic_ratio = ctx->d_fic_ratio; sp.coarse_out = ctx->disable_coarse ? nullptr : ctx->d_coarse; sp.placement = ctx->placement; sp.freqsync = ctx->freqsync;
+    sp.fic_ratio = ctx->d_fic_ratio; sp.coarse_out = ctx->disable_coarse ? nullptr : ctx->d_coarse.get(); sp.placement = ctx->placement; sp.freqsync = ctx->freqsync;
     sp.cir_work = ctx->d_cir_work; sp.search_generic = ctx->search_generic;
     launch_find_index(ctx->dev, sp, ctx->fft_mode, A, 0);
     if ((rc = check_launch(ctx, "find_index_kernel"))) return rc;
@@ -829,14 +918,14 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         launch_find_index(ctx->dev, sp, ctx->fft_mode, A, 2);
         if ((rc = check_launch(ctx, "find_coarse_kernel"))) return rc;
     }
-    post_sync_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, d_index, ctx->disable_coarse ? nullptr : ctx->d_coarse, S, d_prs, d_nco_frame, d_active);
+    post_sync_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, d_index, ctx->disable_coarse ? nullptr : ctx->d_coarse.get(), S, d_prs, d_nco_frame, d_active);
     if ((rc = check_launch(ctx, "post_sync_kernel"))) return rc;
     if (A != A_low) { CK(cudaEventRecord(ctx->evPost, A)); A = A_low; CK(cudaStreamWaitEvent(A, ctx->evPost, 0)); }
     OfdmParams op{}; op.iq = iq; op.stride = stride; op.prs_start = d_prs; op.nco = d_nco_frame; op.active = d_active; op.soft = d_soft; op.soft_stride = DABB_SOFT_PER_FRAME;
     op.r1 = ctx->d_r1; op.freqcorr = d_fc; op.level = d_lvl; op.snr = d_snr; op.n_frames = S; op.groups = ctx->groups; op.sym_per_cta = 75 / ctx->groups;
     op.trace = ctx->trace;
     if (ctx->persistent && !serial) {
-        if (!ctx->d_work && (rc = dalloc(ctx, &ctx->d_work, 1))) return rc;
+        if (!ctx->d_work && (rc = dalloc(ctx, ctx->d_work, 1))) return rc;
         CK(cudaMemsetAsync(ctx->d_work, 0, sizeof(unsigned int), A));
         op.work = ctx->d_work;
     }
@@ -851,7 +940,7 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         null_tap_kernel<<<S, 256, 0, A>>>(scr, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, ctx->d_null);
         if ((rc = check_launch(ctx, "null_tap_kernel"))) return rc;
         if (ctx->decode_tii) {
-            if (!ctx->d_tii && (rc = dalloc(ctx, &ctx->d_tii, (size_t)S * 2 * TU))) return rc;
+            if (!ctx->d_tii && (rc = dalloc(ctx, ctx->d_tii, (size_t)S * 2 * TU))) return rc;
             launch_tii_spectra(ctx->dev, iq, stride, d_prs, d_nco_frame, d_active, ctx->d_null, ctx->d_tii, S, A);
             if ((rc = check_launch(ctx, "tii_spectra_kernel"))) return rc;
         }
@@ -868,23 +957,22 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         auto& sl = ctx->slot[k];
         h_info[k] = sl.d_info;
         if (!sl.configured) continue;
-        const int flen_pad = (sl.flen + 15) & ~15;
         CK(cudaMemsetAsync(sl.d_valid, 0, sizeof(int32_t) * S * 4, B));
-        MscCollectParams cp{}; cp.soft = d_soft; cp.soft_stride = DABB_SOFT_PER_FRAME; cp.active = d_active; cp.slots = ctx->d_slots; cp.n_slots = ctx->n_slots; cp.slot = k; cp.ring = sl.d_ring; cp.ring_pitch = ctx->ring_pitch;
+        MscCollectParams cp{}; cp.soft = d_soft; cp.soft_stride = DABB_SOFT_PER_FRAME; cp.active = d_active; cp.slots = ctx->d_slots; cp.n_slots = ctx->n_slots; cp.slot = k; cp.ring = ctx->d_ring[k]; cp.ring_pitch = ctx->ring_pitch;
         launch_msc_collect(cp, S, B);
         if ((rc = check_launch(ctx, "msc_collect_kernel"))) return rc;
-        MscPrepParams pp{}; pp.active = d_active; pp.slots = ctx->d_slots; pp.n_slots = ctx->n_slots; pp.slot = k; pp.ring = sl.d_ring; pp.ring_pitch = ctx->ring_pitch;
+        MscPrepParams pp{}; pp.active = d_active; pp.slots = ctx->d_slots; pp.n_slots = ctx->n_slots; pp.slot = k; pp.ring = ctx->d_ring[k]; pp.ring_pitch = ctx->ring_pitch;
         pp.frag_out = sl.d_frag; pp.frag_pitch = sl.frag_pitch; pp.valid = sl.d_valid;
         launch_msc_gather(pp, S, B);
         if ((rc = check_launch(ctx, "msc_gather_kernel"))) return rc;
         ViterbiParams vp{}; vp.frag = sl.d_frag; vp.cw_div = 1; vp.outer_stride = sl.frag_pitch; vp.inner_stride = 0; vp.steptab = sl.d_steptab; vp.stage_off = sl.d_stage_off;
         vp.n_cw = S * 4; vp.nsteps = sl.nsteps; vp.nbits = sl.nbits; vp.dec = sl.d_dec;
-        vp.out = sl.d_logical; vp.out_stride = flen_pad; vp.prbs_words = sl.d_prbs_words; vp.valid = sl.d_valid;
+        vp.out = sl.d_logical; vp.out_stride = sl.flen_pad; vp.prbs_words = sl.d_prbs_words; vp.valid = sl.d_valid;
         vp.trace = ctx->trace; vp.trace_kind = 3; vp.split = ctx->vit_split;
         launch_viterbi(vp, B, ctx->vit_stages_now);
         if ((rc = check_launch(ctx, "viterbi_kernel(MSC)"))) return rc;
-        SuperframeParams fp{}; fp.active = d_active; fp.slots = ctx->d_slots; fp.n_slots = ctx->n_slots; fp.slot = k; fp.n_streams = S; fp.logical = sl.d_logical; fp.logical_stride = flen_pad;
-        fp.valid = sl.d_valid; fp.window = sl.d_window; fp.window_pitch = 5 * flen_pad; fp.sf_out = sl.d_sf; fp.sf_pitch = 5 * flen_pad; fp.info = sl.d_info; fp.gf_exp = ctx->dev.gf_exp; fp.gf_log = ctx->dev.gf_log;
+        SuperframeParams fp{}; fp.active = d_active; fp.slots = ctx->d_slots; fp.n_slots = ctx->n_slots; fp.slot = k; fp.n_streams = S; fp.logical = sl.d_logical; fp.logical_stride = sl.flen_pad;
+        fp.valid = sl.d_valid; fp.window = sl.d_window; fp.window_pitch = 5 * sl.flen_pad; fp.sf_out = sl.d_sf; fp.sf_pitch = 5 * sl.flen_pad; fp.info = sl.d_info; fp.gf_exp = ctx->dev.gf_exp; fp.gf_log = ctx->dev.gf_log;
         launch_superframe(fp, B);
         if ((rc = check_launch(ctx, "superframe_kernel"))) return rc;
     }
@@ -897,44 +985,16 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     return DABB_OK;
 }
 
-// logical frames and superframes of the last step: strided device -> host copies (small), into [S][MAX_SUBCH][4][msc_stride] and
-// [S][MAX_SUBCH][sf_stride]; either pointer may be null
-static int copy_logical_frames(dabb_ctx* ctx, uint8_t* msc, int64_t msc_stride, uint8_t* sf, int64_t sf_stride)
-{
-    const int S = ctx->S;
-    for (int k = 0; k < ctx->n_slots; k++) {
-        auto& sl = ctx->slot[k];
-        if (!sl.configured) continue;
-        const int flen_pad = (sl.flen + 15) & ~15;
-        if (msc) {
-            if (msc_stride < sl.flen) { ctx->err = "msc_stride smaller than the logical frame"; return DABB_E_ARG; }
-            // device rows: [S*4][flen_pad] -> host [S][MAX_SUBCH][4][msc_stride]
-            for (int c = 0; c < 4; c++)
-                CK(cudaMemcpy2D(msc + ((size_t)k * 4 + c) * msc_stride, (size_t)DABB_MAX_SUBCH * 4 * msc_stride,
-                                sl.d_logical + (size_t)c * flen_pad, (size_t)4 * flen_pad, sl.flen, S, cudaMemcpyDeviceToHost));
-        }
-        if (sf) {
-            if (sf_stride < 5 * sl.flen) { ctx->err = "sf_stride smaller than the superframe"; return DABB_E_ARG; }
-            CK(cudaMemcpy2D(sf + (size_t)k * sf_stride, (size_t)DABB_MAX_SUBCH * sf_stride,
-                            sl.d_sf, (size_t)5 * flen_pad, 5 * sl.flen, S, cudaMemcpyDeviceToHost));
-        }
-    }
-    return DABB_OK;
-}
-
 int dabb_process(dabb_ctx* ctx, const dabb_io* io)
 {
-    int rc = dabb_process_async(ctx, io);
-    if (rc) return rc;
-    const int S = ctx->S;
-    cudaStream_t B = ctx->prof ? ctx->stream : ctx->streamB;
-    if (io->results) CK(cudaMemcpyAsync(ctx->h_results, ctx->d_results, sizeof(dabb_frame_result) * S, cudaMemcpyDeviceToHost, B));
-    if (io->fibs) CK(cudaMemcpyAsync(ctx->h_fibs, ctx->d_fibs, (size_t)S * 12 * 32, cudaMemcpyDeviceToHost, B));
-    CK(cudaStreamSynchronize(B));
+    if (!ctx || !io) return DABB_E_ARG;
+    cudaSetDevice(ctx->device);
+    const StepOut o = step_out(*io);
+    int rc;
+    if ((rc = check_strides(ctx, o)) || (rc = prepare_pending(ctx, ctx->pend_sync)) || (rc = dabb_process_async(ctx, io)) || (rc = enqueue_readback(ctx, ctx->pend_sync, o)))
+        return rc;
     CK(cudaStreamSynchronize(ctx->stream));
-    if (io->results) memcpy(io->results, ctx->h_results, sizeof(dabb_frame_result) * S);
-    if (io->fibs) memcpy(io->fibs, ctx->h_fibs, (size_t)S * 12 * 32);
-    return copy_logical_frames(ctx, io->msc, io->msc_stride, io->sf, io->sf_stride);
+    return deliver(ctx, ctx->pend_sync);
 }
 
 // ---- pipelined host-buffer path -------------------------------------------------------------------------------------------------
@@ -942,26 +1002,6 @@ int dabb_process(dabb_ctx* ctx, const dabb_io* io)
 // results into one of two pinned result slots on lane B - and return.  dabb_collect: wait for the OLDEST outstanding step and hand
 // its results to the pointers given at submit.  With two steps outstanding the copy of step n+1 overlaps the kernels of step n and
 // the result read-back of step n-1.
-static int ensure_pending(dabb_ctx* ctx, dabb_ctx::Pending& p)
-{
-    const int S = ctx->S;
-    if (!p.done) CK(cudaEventCreateWithFlags(&p.done, cudaEventDisableTiming));
-    if (!p.h_res) CK(cudaHostAlloc((void**)&p.h_res, sizeof(dabb_frame_result) * S, cudaHostAllocDefault));
-    if (!p.h_fibs) CK(cudaHostAlloc((void**)&p.h_fibs, (size_t)S * 12 * 32, cudaHostAllocDefault));
-    size_t msc = 0, sf = 0;
-    for (int k = 0; k < ctx->n_slots; k++) {
-        const auto& sl = ctx->slot[k];
-        p.flen[k] = sl.configured ? sl.flen : 0;
-        if (!sl.configured) continue;
-        const size_t fp = (size_t)((sl.flen + 15) & ~15);
-        p.msc_off[k] = msc; p.sf_off[k] = sf;
-        msc += (size_t)S * 4 * fp; sf += (size_t)S * 5 * fp;
-    }
-    if (msc > p.msc_bytes) { if (p.h_msc) cudaFreeHost(p.h_msc); p.h_msc = nullptr; CK(cudaHostAlloc((void**)&p.h_msc, msc, cudaHostAllocDefault)); p.msc_bytes = msc; }
-    if (sf > p.sf_bytes) { if (p.h_sf) cudaFreeHost(p.h_sf); p.h_sf = nullptr; CK(cudaHostAlloc((void**)&p.h_sf, sf, cudaHostAllocDefault)); p.sf_bytes = sf; }
-    return DABB_OK;
-}
-
 int dabb_submit(dabb_ctx* ctx, const dabb_io* io)
 {
     if (!ctx || !io || !io->iq || !io->buf_start || !io->iq_is_host) return DABB_E_ARG;
@@ -970,24 +1010,22 @@ int dabb_submit(dabb_ctx* ctx, const dabb_io* io)
     cudaSetDevice(ctx->device);
     const int S = ctx->S, fmt = io->iq_format;
     if (fmt < 0 || fmt > DABB_IQ_S16BE) { ctx->err = "unknown iq_format"; return DABB_E_ARG; }
+    const StepOut o = step_out(*io);
     int rc;
+    if ((rc = check_strides(ctx, o))) return rc;
     if (!ctx->streamC) {
         CK(cudaStreamCreateWithFlags(&ctx->streamC, cudaStreamNonBlocking));
         for (int i = 0; i < 2; i++) { CK(cudaEventCreateWithFlags(&ctx->evH2D[i], cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&ctx->evStageFree[i], cudaEventDisableTiming)); }
     }
     const int slot = (int)(ctx->submits & 1);
     dabb_ctx::Pending& p = ctx->pend[(ctx->pend_head + ctx->pend_count) & 1];
-    if ((rc = ensure_pending(ctx, p))) return rc;
-    cudaStream_t A = ctx->stream, B = ctx->streamB, Cs = ctx->streamC;
-    const size_t bps = fmt == DABB_IQ_CF32 ? 8 : ((fmt == DABB_IQ_U8 || fmt == DABB_IQ_S8) ? 2 : 4);
+    if ((rc = prepare_pending(ctx, p))) return rc;
+    cudaStream_t A = ctx->stream, Cs = ctx->streamC;
+    const size_t bps = bytes_per_sample(fmt);
     const size_t need = (size_t)S * io->buf_len * bps;
-    if (need > ctx->stage2_bytes[slot]) {
-        sync_all(ctx); cudaStreamSynchronize(Cs);
-        if (ctx->d_stage2[slot]) cudaFree(ctx->d_stage2[slot]);
-        ctx->d_stage2[slot] = nullptr; ctx->stage2_bytes[slot] = 0;
-        cudaError_t e = cudaMalloc(&ctx->d_stage2[slot], need);
-        if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc(pipelined staging): ") + cudaGetErrorString(e); return DABB_E_NOMEM; }
-        ctx->stage2_bytes[slot] = need; ctx->stageFreeValid[slot] = false;
+    if (need > ctx->d_stage2[slot].size()) {
+        if ((rc = grow(ctx, ctx->d_stage2[slot], need))) return rc;
+        ctx->stageFreeValid[slot] = false;
     }
     // the staging slot was last read by the step submitted two calls ago
     if (ctx->stageFreeValid[slot]) CK(cudaStreamWaitEvent(Cs, ctx->evStageFree[slot], 0));
@@ -999,52 +1037,24 @@ int dabb_submit(dabb_ctx* ctx, const dabb_io* io)
         }
         for (int s = 0; s < S; s++)
             if (io->buf_start[s] != ctx->stage_last_start[s] + ctx->stage_last_len - carry) { ctx->err = "carry_samples: a window does not start where the previous one ended minus the carry"; return DABB_E_ARG; }
-        const unsigned char* prev = reinterpret_cast<const unsigned char*>(ctx->d_stage2[slot ^ 1]);
+        const uint8_t* prev = ctx->d_stage2[slot ^ 1];
         CK(cudaMemcpy2DAsync(ctx->d_stage2[slot], (size_t)io->buf_len * bps, prev + (size_t)(ctx->stage_last_len - carry) * bps, (size_t)ctx->stage_last_len * bps,
                              (size_t)carry * bps, S, cudaMemcpyDeviceToDevice, Cs));          // same stream as the copy that filled the other slot
     }
-    CK(cudaMemcpy2DAsync(reinterpret_cast<unsigned char*>(ctx->d_stage2[slot]) + (size_t)carry * bps, (size_t)io->buf_len * bps,
+    CK(cudaMemcpy2DAsync(ctx->d_stage2[slot] + (size_t)carry * bps, (size_t)io->buf_len * bps,
                          reinterpret_cast<const unsigned char*>(io->iq) + (size_t)carry * bps, (size_t)io->stride_samples * bps, (size_t)(io->buf_len - carry) * bps, S, cudaMemcpyHostToDevice, Cs));
     ctx->stage_last_fmt = fmt; ctx->stage_last_len = io->buf_len; ctx->stage_last_start.assign(io->buf_start, io->buf_start + S);
     CK(cudaEventRecord(ctx->evH2D[slot], Cs));
     CK(cudaStreamWaitEvent(A, ctx->evH2D[slot], 0));
-    const float2* iq = reinterpret_cast<const float2*>(ctx->d_stage2[slot]);
+    const float2* iq = reinterpret_cast<const float2*>(ctx->d_stage2[slot].get());
     if (fmt != DABB_IQ_CF32) {
-        const size_t ns = (size_t)S * io->buf_len;
-        if (ns > ctx->iq_stage_samples) {
-            sync_all(ctx);
-            if (ctx->d_iq_stage) cudaFree(ctx->d_iq_stage);
-            ctx->d_iq_stage = nullptr; ctx->iq_stage_samples = 0;
-            cudaError_t e = cudaMalloc((void**)&ctx->d_iq_stage, ns * sizeof(float2));
-            if (e != cudaSuccess) { ctx->err = std::string("cudaMalloc(iq staging): ") + cudaGetErrorString(e); return DABB_E_NOMEM; }
-            ctx->iq_stage_samples = ns;
-        }
-        const dim3 grid((unsigned)((io->buf_len + 255) / 256), (unsigned)S);
-        convert_iq_kernel<<<grid, 256, 0, A>>>(reinterpret_cast<const uint8_t*>(ctx->d_stage2[slot]), io->buf_len, fmt, ctx->d_iq_stage, io->buf_len, io->buf_len, S);
-        if ((rc = check_launch(ctx, "convert_iq_kernel"))) return rc;
+        if ((rc = convert_to_stage(ctx, ctx->d_stage2[slot], io->buf_len, fmt, io->buf_len))) return rc;
         CK(cudaEventRecord(ctx->evStageFree[slot], A)); ctx->stageFreeValid[slot] = true;       // the raw bytes are consumed
         iq = ctx->d_iq_stage;
     }
     if ((rc = enqueue_step(ctx, io, iq, io->buf_len))) return rc;
     if (fmt == DABB_IQ_CF32) { CK(cudaEventRecord(ctx->evStageFree[slot], A)); ctx->stageFreeValid[slot] = true; }   // lane A has read the samples
-    // results -> pinned slot, on lane B behind the step's result record
-    if (io->results) CK(cudaMemcpyAsync(p.h_res, ctx->d_results, sizeof(dabb_frame_result) * S, cudaMemcpyDeviceToHost, B));
-    if (io->fibs) CK(cudaMemcpyAsync(p.h_fibs, ctx->d_fibs, (size_t)S * 12 * 32, cudaMemcpyDeviceToHost, B));
-    for (int k = 0; k < ctx->n_slots; k++) {
-        const auto& sl = ctx->slot[k];
-        if (!sl.configured) continue;
-        const size_t fp = (size_t)((sl.flen + 15) & ~15);
-        if (io->msc) {
-            if (io->msc_stride < sl.flen) { ctx->err = "msc_stride smaller than the logical frame"; return DABB_E_ARG; }
-            CK(cudaMemcpyAsync(p.h_msc + p.msc_off[k], sl.d_logical, (size_t)S * 4 * fp, cudaMemcpyDeviceToHost, B));
-        }
-        if (io->sf) {
-            if (io->sf_stride < 5 * sl.flen) { ctx->err = "sf_stride smaller than the superframe"; return DABB_E_ARG; }
-            CK(cudaMemcpyAsync(p.h_sf + p.sf_off[k], sl.d_sf, (size_t)S * 5 * fp, cudaMemcpyDeviceToHost, B));
-        }
-    }
-    CK(cudaEventRecord(p.done, B));
-    p.io = *io; p.used = true;
+    if ((rc = enqueue_readback(ctx, p, o))) return rc;
     ctx->pend_count++; ctx->submits++;
     return DABB_OK;
 }
@@ -1054,23 +1064,8 @@ int dabb_collect(dabb_ctx* ctx)
     if (!ctx) return DABB_E_ARG;
     if (ctx->pend_count == 0) { ctx->err = "nothing outstanding"; return DABB_E_STATE; }
     cudaSetDevice(ctx->device);
-    dabb_ctx::Pending& p = ctx->pend[ctx->pend_head];
-    CK(cudaEventSynchronize(p.done));
-    const int S = ctx->S;
-    const dabb_io& io = p.io;
-    if (io.results) memcpy(io.results, p.h_res, sizeof(dabb_frame_result) * S);
-    if (io.fibs) memcpy(io.fibs, p.h_fibs, (size_t)S * 12 * 32);
-    for (int k = 0; k < ctx->n_slots; k++) {
-        const int flen = p.flen[k];
-        if (!flen) continue;
-        const size_t fp = (size_t)((flen + 15) & ~15);
-        if (io.msc)       // pinned rows [S*4][fp] -> caller [S][MAX_SUBCH][4][msc_stride]
-            for (int s = 0; s < S; s++) for (int c = 0; c < 4; c++)
-                memcpy(io.msc + (((size_t)s * DABB_MAX_SUBCH + k) * 4 + c) * io.msc_stride, p.h_msc + p.msc_off[k] + ((size_t)s * 4 + c) * fp, (size_t)flen);
-        if (io.sf)
-            for (int s = 0; s < S; s++) memcpy(io.sf + ((size_t)s * DABB_MAX_SUBCH + k) * io.sf_stride, p.h_sf + p.sf_off[k] + (size_t)s * 5 * fp, (size_t)5 * flen);
-    }
-    p.used = false;
+    int rc;
+    if ((rc = deliver(ctx, ctx->pend[ctx->pend_head]))) return rc;
     ctx->pend_head ^= 1; ctx->pend_count--;
     return DABB_OK;
 }
@@ -1121,7 +1116,11 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
     if (what == 6) { const size_t n = (size_t)ctx->S * 12 * 32; CK(cudaMemcpy(host_out, ctx->d_fibs, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 7 || what == 8) {      // the layouts of dabb_io.msc / dabb_io.sf, the stride implied by `bytes`
         const int64_t per = (int64_t)ctx->S * DABB_MAX_SUBCH * (what == 7 ? 4 : 1), stride = (int64_t)(bytes / (size_t)per);
-        return what == 7 ? copy_logical_frames(ctx, (uint8_t*)host_out, stride, nullptr, 0) : copy_logical_frames(ctx, nullptr, 0, (uint8_t*)host_out, stride);
+        uint8_t* out = (uint8_t*)host_out;
+        const StepOut o = what == 7 ? StepOut{nullptr, nullptr, out, stride, nullptr, 0} : StepOut{nullptr, nullptr, nullptr, 0, out, stride};
+        int rc;
+        if ((rc = check_strides(ctx, o)) || (rc = prepare_pending(ctx, ctx->pend_sync)) || (rc = enqueue_readback(ctx, ctx->pend_sync, o))) return rc;
+        return deliver(ctx, ctx->pend_sync);
     }
     ctx->err = "tap not available (keep_taps = 0?)";
     return DABB_E_STATE;
@@ -1136,19 +1135,20 @@ int dabb_ofdm_demod(dabb_ctx* ctx, const float* iq, int64_t stride, const int64_
     OfdmParams op{}; op.iq = reinterpret_cast<const float2*>(iq); op.stride = stride; op.prs_start = prs_start; op.active = nullptr; op.soft = soft; op.soft_stride = DABB_SOFT_PER_FRAME;
     op.r1 = reinterpret_cast<float2*>(r1); op.freqcorr = reinterpret_cast<float2*>(fc); op.snr = nullptr; op.n_frames = n;
     op.groups = (fc || n >= 1024) ? 1 : (n >= 64 ? 5 : 25); op.sym_per_cta = 75 / op.groups; op.n_full = n; op.tail_groups = 1; op.fc_pitch = op.groups; op.nco_fast = ctx->nco_fast;
-    int32_t* nco4 = nullptr;
+    DevBuf<int32_t> nco4;
+    int rc;
     if (nco) {
         // expand {lp applied to PRS sample 0, Hz} to the 4-entry form of the pipeline (same increment for PRS and symbols)
         std::vector<int32_t> h(2 * (size_t)n), h4(4 * (size_t)n);
         CK(cudaMemcpy(h.data(), nco, sizeof(int32_t) * 2 * n, cudaMemcpyDeviceToHost));
         for (int i = 0; i < n; i++) { h4[4 * i] = h[2 * i]; h4[4 * i + 1] = h[2 * i + 1]; h4[4 * i + 2] = h[2 * i]; h4[4 * i + 3] = h[2 * i + 1]; }
-        CK(cudaMalloc((void**)&nco4, sizeof(int32_t) * 4 * n));
+        if ((rc = dalloc(ctx, nco4, 4 * (size_t)n, false))) return rc;
         CK(cudaMemcpy(nco4, h4.data(), sizeof(int32_t) * 4 * n, cudaMemcpyHostToDevice));
         op.nco = nco4;
     }
     launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, ctx->stream);
-    int rc = check_launch(ctx, "ofdm_demod_kernel");
-    if (nco4) { cudaStreamSynchronize(ctx->stream); cudaFree(nco4); }
+    rc = check_launch(ctx, "ofdm_demod_kernel");
+    if (nco4) cudaStreamSynchronize(ctx->stream);
     return rc;
 }
 
@@ -1159,13 +1159,13 @@ int dabb_find_index_ex(dabb_ctx* ctx, const float* iq, int64_t stride, const int
     sync_all(ctx);
     SyncParams sp{}; sp.iq = reinterpret_cast<const float2*>(iq); sp.stride = stride; sp.win_start = win_start; sp.nco = nullptr; sp.active = nullptr; sp.index_out = index_out; sp.cir_out = cir_out; sp.n = n; sp.fic_ratio = nullptr; sp.coarse_out = nullptr; sp.placement = placement; sp.freqsync = 0;
     // magnitudes between the transform and the search kernel: the context's buffer when the batch fits, else a temporary
-    float* work = n <= ctx->S ? ctx->d_cir_work : nullptr;
-    bool temp = false;
-    if (!work) { if (cudaMalloc((void**)&work, (size_t)n * TU * sizeof(float)) != cudaSuccess) { ctx->err = "cudaMalloc(findIndex work buffer)"; return DABB_E_NOMEM; } temp = true; }
-    sp.cir_work = work; sp.search_generic = ctx->search_generic;
+    DevBuf<float> temp;
+    int rc;
+    if (n > ctx->S && (rc = dalloc(ctx, temp, (size_t)n * TU, false))) return rc;
+    sp.cir_work = temp ? temp.get() : ctx->d_cir_work.get(); sp.search_generic = ctx->search_generic;
     launch_find_index(ctx->dev, sp, ctx->fft_mode, ctx->stream);
-    int rc = check_launch(ctx, "find_index_kernel");
-    if (temp) { cudaStreamSynchronize(ctx->stream); cudaFree(work); }
+    rc = check_launch(ctx, "find_index_kernel");
+    if (temp) cudaStreamSynchronize(ctx->stream);
     return rc;
 }
 
@@ -1210,19 +1210,18 @@ static int run_stage_viterbi(dabb_ctx* ctx, const int8_t* soft, int n_cw, int64_
     build_vit_tables_u2(map, nsteps, steps, soff);
     if ((int)soff.back() > frag) { ctx->err = "de-puncturing map consumes more softbits than provided"; return DABB_E_ARG; }
     const int pitch = (frag + 15) & ~15;
-    uint2* d_steps = nullptr; uint32_t* d_soff = nullptr; int8_t* tmp = nullptr;
-    CK(cudaMalloc((void**)&d_steps, steps.size() * sizeof(uint2))); CK(cudaMalloc((void**)&d_soff, soff.size() * 4));
-    CK(cudaMalloc((void**)&tmp, (size_t)n_cw * pitch + VIT_FRAG_SLACK));
+    DevBuf<uint2> d_steps; DevBuf<uint32_t> d_soff; DevBuf<int8_t> tmp;
+    int rc;
+    if ((rc = dalloc(ctx, d_steps, steps.size(), false)) || (rc = dalloc(ctx, d_soff, soff.size(), false)) || (rc = dalloc(ctx, tmp, (size_t)n_cw * pitch + VIT_FRAG_SLACK, false))) return rc;
     CK(cudaMemcpyAsync(d_steps, steps.data(), steps.size() * sizeof(uint2), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(d_soff, soff.data(), soff.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemsetAsync(tmp, 0, (size_t)n_cw * pitch + VIT_FRAG_SLACK, ctx->stream));
-    int rc = 0;
     if (pitch == frag && in_stride == frag) { launch_clamp_copy(soft, tmp, (int64_t)n_cw * frag, ctx->stream); rc = check_launch(ctx, "clamp_copy_kernel"); }
     else {
         CK(cudaMemcpy2DAsync(tmp, pitch, soft, (size_t)in_stride, frag, n_cw, cudaMemcpyDeviceToDevice, ctx->stream));
         launch_clamp_copy(tmp, tmp, (int64_t)n_cw * pitch, ctx->stream); rc = check_launch(ctx, "clamp_copy_kernel");
     }
-    if (!rc) rc = ensure_dec(ctx, vit_dec_bytes(n_cw, nsteps));
+    if (!rc) rc = grow(ctx, ctx->d_dec, vit_dec_bytes(n_cw, nsteps) / sizeof(uint2));
     if (!rc) {
         ViterbiParams vp{}; vp.frag = tmp; vp.cw_div = 1; vp.outer_stride = pitch; vp.inner_stride = 0; vp.steptab = d_steps; vp.stage_off = d_soff;
         vp.n_cw = n_cw; vp.nsteps = nsteps; vp.nbits = nbits; vp.dec = ctx->d_dec; vp.out = out; vp.out_stride = out_stride; vp.prbs_words = d_prbs_words; vp.valid = nullptr;
@@ -1230,7 +1229,6 @@ static int run_stage_viterbi(dabb_ctx* ctx, const int8_t* soft, int n_cw, int64_
         rc = check_launch(ctx, "viterbi_kernel");
     }
     cudaStreamSynchronize(ctx->stream);
-    cudaFree(d_steps); cudaFree(d_soff); cudaFree(tmp);
     return rc;
 }
 
@@ -1240,14 +1238,14 @@ int dabb_viterbi(dabb_ctx* ctx, const int8_t* soft, int32_t n_cw, int32_t nbits,
     cudaSetDevice(ctx->device);
     sync_all(ctx);
     const int nsteps = nbits + 6, ob = nbits / 8;
-    uint8_t* bytes = nullptr;
-    CK(cudaMalloc((void**)&bytes, (size_t)n_cw * ob));
+    DevBuf<uint8_t> bytes;
+    int rc;
+    if ((rc = dalloc(ctx, bytes, (size_t)n_cw * ob, false))) return rc;
     std::vector<int16_t> map((size_t)nsteps * 4);
     std::fill(map.begin(), map.end(), (int16_t)0);                      // >= 0 = present: nothing punctured, the caller's zeros are softbit 0
-    int rc = run_stage_viterbi(ctx, soft, n_cw, (int64_t)nsteps * 4, nsteps * 4, map.data(), nsteps, nbits, nullptr, bytes, ob);
+    rc = run_stage_viterbi(ctx, soft, n_cw, (int64_t)nsteps * 4, nsteps * 4, map.data(), nsteps, nbits, nullptr, bytes, ob);
     if (!rc) { launch_unpack_bits(bytes, ob, n_cw, nbits, bits_out, ctx->stream); rc = check_launch(ctx, "unpack_bits_kernel"); }
     cudaStreamSynchronize(ctx->stream);
-    cudaFree(bytes);
     return rc;
 }
 
@@ -1275,13 +1273,13 @@ int dabb_msc_decode(dabb_ctx* ctx, const dabb_subchannel* sc, const int8_t* soft
     std::vector<int16_t> map((size_t)nsteps * 4);
     build_msc_map(*ctx->host, prof, map.data());
     std::vector<uint32_t> w; pack_prbs_words(ctx->host->prbs, nbits, w);
-    uint32_t* d_w = nullptr;
-    CK(cudaMalloc((void**)&d_w, w.size() * 4));
+    DevBuf<uint32_t> d_w;
+    int rc;
+    if ((rc = dalloc(ctx, d_w, w.size(), false))) return rc;
     CK(cudaMemcpy(d_w, w.data(), w.size() * 4, cudaMemcpyHostToDevice));
     // output rows are 3*bitrate bytes (a multiple of 4)
-    int rc = run_stage_viterbi(ctx, soft, n, frag, frag, map.data(), nsteps, nbits, d_w, bytes_out, flen);
+    rc = run_stage_viterbi(ctx, soft, n, frag, frag, map.data(), nsteps, nbits, d_w, bytes_out, flen);
     cudaStreamSynchronize(ctx->stream);
-    cudaFree(d_w);
     return rc;
 }
 
