@@ -79,9 +79,29 @@ typedef struct {
     int32_t disable_coarse;
     int32_t fft_placement;      /* DABB_PLACEMENT_* */
     int32_t freqsync_method;    /* DABB_FREQSYNC_* */
-    int32_t decode_tii;         /* RadioReceiverOptions::decodeTII: with keep_taps, also produce tap 4 (the two spectra TIIDecoder starts from) */
+    int32_t decode_tii;         /* RadioReceiverOptions::decodeTII: analyse the transmitter identification of every decoded frame on the device
+                                   (tap 9); with keep_taps, also produce tap 4 (the two spectra TIIDecoder starts from) */
     int32_t reserved[4];
 } dabb_options;
+
+/* Transmitter identification (TIIDecoder, backend/tii-decoder.cpp:236-383) of one stream in one step: tap 9.  Every decoded frame is
+ * analysed while dabb_options.decode_tii is set; each (comb, pattern) combination found in a frame accumulates its phase-error table over
+ * five analyses and is then reported once, like onTIIMeasurement.  A frame reports at most DABB_TII_MAX combinations (the reference
+ * skips frames with 10 or more); within a record they are in ascending (comb, pattern) order (the reference's order within a frame is
+ * that of an unordered_map).  A stream keeps at most 32 combinations open: a new one beyond that replaces the least recently analysed
+ * one, which then starts over (`evicted`).  dabb_stream_reset clears a stream's combinations; switching decode_tii off keeps them. */
+enum { DABB_TII_MAX = 9 };
+typedef struct {
+    int32_t count;              /* measurements reported in this step (0..DABB_TII_MAX) */
+    int32_t evicted;            /* open combinations replaced in this step */
+    int32_t skipped;            /* 1: the frame was decoded but not analysed (10 or more likely combinations) */
+    int32_t reserved;
+    struct {
+        int32_t comb, pattern;  /* tii_measurement_t::comb, pattern */
+        int32_t delay_samples;  /* delay hypothesis -4 .. 499 with the smallest accumulated phase error */
+        float error;            /* that accumulated error (integer valued) */
+    } m[DABB_TII_MAX];
+} dabb_tii_result;
 
 /* replaces: RadioReceiver::RadioReceiver / ~RadioReceiver (backend/radio-receiver.h:52-116) */
 int dabb_create(const dabb_config* cfg, dabb_ctx** out);
@@ -203,12 +223,14 @@ int dabb_profile_read(dabb_ctx* ctx, char* json_out, size_t cap);
  *   3 = null symbol cf32 [n_streams][2656], NCO applied  onNewNullSymbol (ofdm-processor.cpp:462-469)
  *   4 = TII spectra cf32 [n_streams][2][2048] (only while dabb_options.decode_tii is set): fft::Forward of the frame's phase
  *       reference symbol and of the last T_u samples of the null symbol that follows it, what TIIDecoder::run computes first
- *       (tii-decoder.cpp:197-214); the pattern analysis itself is host work (welle.io_b200/host/tii.h)
+ *       (tii-decoder.cpp:197-214); tap 9 is the analysis of these spectra
  * and, with any keep_taps, what the last step of dabb_process_async left on the device, the outputs dabb_process would have returned:
  *   5 = dabb_frame_result [n_streams]
  *   6 = FIBs uint8 [n_streams][12][32]
  *   7 = logical frames uint8 [n_streams][DABB_MAX_SUBCH][4][stride], the layout of dabb_io.msc; stride = bytes / (n_streams * DABB_MAX_SUBCH * 4)
- *   8 = DAB+ superframes uint8 [n_streams][DABB_MAX_SUBCH][stride], the layout of dabb_io.sf; stride = bytes / (n_streams * DABB_MAX_SUBCH) */
+ *   8 = DAB+ superframes uint8 [n_streams][DABB_MAX_SUBCH][stride], the layout of dabb_io.sf; stride = bytes / (n_streams * DABB_MAX_SUBCH)
+ *   9 = dabb_tii_result [n_streams] of the last step (all zero when that step ran with decode_tii off); DABB_E_STATE until
+ *       dabb_options.decode_tii has been set once */
 int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes);
 
 /* ---------------------------------------------------------------------------------------------------------

@@ -90,7 +90,12 @@ struct dabb_ctx {
     int64_t step = 0; int last_parity = 0; DevBuf<int32_t> d_fic_ratio, d_coarse; int ofdm_smem_floor = 0; int vit_stages_now = 3;
     int prio_b = 0; cudaStream_t streamP = nullptr; cudaEvent_t evPre = nullptr, evPost = nullptr;      // time-sync kernels of lane A at the highest priority (see dabb_create)
     cudaStream_t stream2 = nullptr; cudaEvent_t ev_ofdm = nullptr, ev_fic = nullptr; DevBuf<uint2> d_dec_fic; int S = 0; int fft_mode = 0; int disable_coarse = 0; int keep_taps = 0; int placement = 0; int freqsync = 0;
-    int decode_tii = 0; DevBuf<float2> d_tii; bool persistent = false; DevBuf<unsigned int> d_work; TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0; int flen_max = 0;
+    int decode_tii = 0; DevBuf<float2> d_tii;
+    // TII analysis (tii.cu), allocated when decode_tii is first set: the null symbol when keep_taps has no tap for it, each stream's open
+    // combinations and their phase-error sums, the step's analyses, the tie-order tables and the step's records (tap 9)
+    DevBuf<float2> d_tii_null; DevBuf<dabb_tii::StreamHdr> d_tii_hdr; DevBuf<dabb_tii::Job> d_tii_jobs; DevBuf<int32_t> d_tii_njobs;
+    DevBuf<uint32_t> d_tii_sums; DevBuf<uint16_t> d_tii_rank; DevBuf<dabb_tii_result> d_tii_res;
+    bool persistent = false; DevBuf<unsigned int> d_work; TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0; int flen_max = 0;
     DevBuf<unsigned long long> d_trace_rec; DevBuf<unsigned int> d_trace_count;      // what `trace` points into
     std::string err; int64_t launches = 0; int osc_mismatches = -1; int osc_patched = 0; std::vector<float2> h_osc;
     HostTables* host = nullptr; DevTables dev{};
@@ -748,6 +753,7 @@ int dabb_stream_reset(dabb_ctx* ctx, int32_t first, int32_t count, int64_t pos)
     cudaSetDevice(ctx->device);
     sync_all(ctx);
     reset_kernel<<<(count + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_state, ctx->d_slots, ctx->n_slots, first, count, pos, ctx->d_fic_ratio);
+    if (ctx->d_tii_hdr) CK(cudaMemsetAsync(ctx->d_tii_hdr + first, 0, sizeof(dabb_tii::StreamHdr) * count, ctx->stream));     // no open TII combinations
     for (int i = first; i < first + count; i++) for (int k = 0; k < ctx->n_slots; k++) { ctx->h_slots[(size_t)i * ctx->n_slots + k].cif_count = 0; ctx->h_slots[(size_t)i * ctx->n_slots + k].sf_frame_count = 0; }
     { int rc_ = check_launch(ctx, "reset_kernel"); cudaStreamSynchronize(ctx->stream); ctx->evB_valid[0] = ctx->evB_valid[1] = false; return rc_; }
 }
@@ -936,15 +942,24 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     if ((rc = check_launch(ctx, "ofdm_demod_kernel"))) return rc;
     advance_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, S, ctx->fc_pitch, d_fc, d_lvl);
     if ((rc = check_launch(ctx, "advance_kernel"))) return rc;
-    if (ctx->d_null) {
-        null_tap_kernel<<<S, 256, 0, A>>>(scr, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, ctx->d_null);
+    // the null symbol: tap 3 with keep_taps, else (TII only) an internal buffer
+    float2* d_null = ctx->d_null ? ctx->d_null.get() : (ctx->decode_tii ? ctx->d_tii_null.get() : nullptr);
+    if (d_null) {
+        null_tap_kernel<<<S, 256, 0, A>>>(scr, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, d_null);
         if ((rc = check_launch(ctx, "null_tap_kernel"))) return rc;
         if (ctx->decode_tii) {
             if (!ctx->d_tii && (rc = dalloc(ctx, ctx->d_tii, (size_t)S * 2 * TU))) return rc;
-            launch_tii_spectra(ctx->dev, iq, stride, d_prs, d_nco_frame, d_active, ctx->d_null, ctx->d_tii, S, A);
+            launch_tii_spectra(ctx->dev, iq, stride, d_prs, d_nco_frame, d_active, d_null, ctx->d_tii, S, A);
             if ((rc = check_launch(ctx, "tii_spectra_kernel"))) return rc;
+            TiiParams tp{}; tp.spectra = ctx->d_tii; tp.active = d_active; tp.hdr = ctx->d_tii_hdr; tp.jobs = ctx->d_tii_jobs; tp.njobs = ctx->d_tii_njobs;
+            tp.sums = ctx->d_tii_sums; tp.rank = ctx->d_tii_rank; tp.res = ctx->d_tii_res.get(); tp.n = S;
+            launch_tii_plan(tp, A);
+            if ((rc = check_launch(ctx, "tii_plan_kernel"))) return rc;
+            launch_tii_phase(tp, A);
+            if ((rc = check_launch(ctx, "tii_phase_kernel"))) return rc;
         }
     }
+    if (!ctx->decode_tii && ctx->d_tii_res) CK(cudaMemsetAsync(ctx->d_tii_res, 0, sizeof(dabb_tii_result) * S, A));     // tap 9: nothing analysed in this step
     if (!serial) { CK(cudaEventRecord(ctx->evA[par], A)); CK(cudaStreamWaitEvent(B, ctx->evA[par], 0)); }
     // ---------------- lane B: FIC chain forked onto its own stream, MSC chain per slot (longest first), then the result record.
     // (One fused Viterbi launch over FIC + MSC codewords was measured slower: 1.44 ms vs 0.34 + 1.02 ms.)
@@ -1110,7 +1125,11 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
         CK(cudaMemcpy2D(host_out, 8, ctx->d_r1, 96 * 8, 8, n, cudaMemcpyDeviceToHost));
         return 0;
     }
-    if (what == 4 && ctx->d_tii && ctx->decode_tii) { const size_t n = (size_t)ctx->S * 2 * TU * 8; CK(cudaMemcpy(host_out, ctx->d_tii, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
+    if (what == 9) {
+        if (!ctx->d_tii_res) { ctx->err = "tap 9 needs dabb_options.decode_tii to have been set"; return DABB_E_STATE; }
+        const size_t n = sizeof(dabb_tii_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_tii_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
+    }
+    if (what == 4 && ctx->d_tii && ctx->d_null && ctx->decode_tii) { const size_t n = (size_t)ctx->S * 2 * TU * 8; CK(cudaMemcpy(host_out, ctx->d_tii, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 3 && ctx->d_null) { const size_t n = (size_t)ctx->S * TNULL * 8; CK(cudaMemcpy(host_out, ctx->d_null, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 5) { const size_t n = sizeof(dabb_frame_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_results, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 6) { const size_t n = (size_t)ctx->S * 12 * 32; CK(cudaMemcpy(host_out, ctx->d_fibs, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
@@ -1197,6 +1216,22 @@ int dabb_get_info(dabb_ctx* ctx, int32_t what, int64_t* out)
 int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
 {
     if (!ctx || !opt || opt->fft_placement < 0 || opt->fft_placement > 2 || opt->freqsync_method < 0 || opt->freqsync_method > 2) return DABB_E_ARG;
+    if (opt->decode_tii && !ctx->d_tii_res) {       // first use of TII: its buffers (64 KB per stream), zeroed = no open combinations
+        cudaSetDevice(ctx->device);
+        sync_all(ctx);
+        const size_t S = (size_t)ctx->S;
+        uint16_t rank[2][dabb_tii::N_ERR];
+        dabb_tii::build_rank_tables(rank);
+        int rc;
+        if ((!ctx->d_null && (rc = dalloc(ctx, ctx->d_tii_null, S * TNULL))) || (rc = dalloc(ctx, ctx->d_tii_hdr, S)) || (rc = dalloc(ctx, ctx->d_tii_jobs, S * dabb_tii::MAX_JOBS)) ||
+            (rc = dalloc(ctx, ctx->d_tii_njobs, S)) || (rc = dalloc(ctx, ctx->d_tii_sums, S * dabb_tii::N_SLOTS * dabb_tii::N_ERR)) || (rc = dalloc(ctx, ctx->d_tii_rank, 2 * dabb_tii::N_ERR))) {
+            ctx->d_tii_null.reset(); ctx->d_tii_hdr.reset(); ctx->d_tii_jobs.reset(); ctx->d_tii_njobs.reset(); ctx->d_tii_sums.reset(); ctx->d_tii_rank.reset();
+            return rc;
+        }
+        CK(cudaMemcpyAsync(ctx->d_tii_rank, rank, sizeof rank, cudaMemcpyHostToDevice, ctx->stream));
+        if ((rc = dalloc(ctx, ctx->d_tii_res, S))) return rc;      // last: it marks the analysis as available
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
     ctx->disable_coarse = opt->disable_coarse != 0; ctx->placement = opt->fft_placement; ctx->freqsync = opt->freqsync_method; ctx->decode_tii = opt->decode_tii != 0;
     return DABB_OK;
 }

@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <string>
 #include "ofdm_core.cuh"
+#include "tii_core.cuh"
 
 namespace dabb {
 
@@ -81,6 +82,20 @@ void launch_find_index(const DevTables& tb, const SyncParams& p, int fft_mode, c
 void launch_tii_spectra(const DevTables& tb, const float2* iq, int64_t stride, const int64_t* prs_start, const int32_t* nco_frame, const int32_t* active,
                         const float2* nulls, float2* out, int n, cudaStream_t st);
 void launch_coarse(const DevTables& tb, const float2* iq, int64_t stride, const int64_t* prs_start, int n, int freqsync, int32_t* out, cudaStream_t st);
+
+// ---- TII analysis (tii.cu, tii_core.cuh) ----
+struct TiiParams {
+    const float2* spectra;                       // [n][2][T_u] from tii_spectra_kernel: phase reference symbol, null symbol
+    const int32_t* active;                       // [n] 1 = the stream decoded a frame in this step
+    dabb_tii::StreamHdr* hdr;                    // [n] open combinations
+    dabb_tii::Job* jobs; int32_t* njobs;         // [n][MAX_JOBS], [n]: this step's analyses (tii_plan_kernel -> tii_phase_kernel)
+    uint32_t* sums;                              // [n][N_SLOTS][N_ERR] accumulated phase errors
+    const uint16_t* rank;                        // [2][N_ERR] arg-min tie order (dabb_tii::build_rank_tables)
+    void* res;                                   // [n] dabb_tii_result
+    int n;
+};
+void launch_tii_plan(const TiiParams& p, cudaStream_t st);
+void launch_tii_phase(const TiiParams& p, cudaStream_t st);
 
 // ---- host-side table builders (tables.cpp) ----
 struct HostTables {

@@ -61,6 +61,12 @@ RESULT_DTYPE = np.dtype([("status", "<i4"), ("start_index", "<i4"), ("fine_corr"
                          ("slevel", "<f4"), ("acq_failed", "<i4"), ("reserved", "<i4", (2,))], align=True)
 assert RESULT_DTYPE.itemsize == C.sizeof(FrameResult), (RESULT_DTYPE.itemsize, C.sizeof(FrameResult))
 
+TII_MAX = 9
+# dabb_tii_result: one stream's transmitter identification measurements of one step (tap 9)
+TII_DTYPE = np.dtype([("count", "<i4"), ("evicted", "<i4"), ("skipped", "<i4"), ("reserved", "<i4"),
+                      ("m", [("comb", "<i4"), ("pattern", "<i4"), ("delay_samples", "<i4"), ("error", "<f4")], (TII_MAX,))])
+assert TII_DTYPE.itemsize == 16 + 16 * TII_MAX
+
 
 class IO(C.Structure):
     _fields_ = [("iq", C.c_void_p), ("iq_is_host", C.c_int32), ("stride_samples", C.c_int64), ("buf_start", C.c_void_p), ("buf_len", C.c_int64),
@@ -299,8 +305,8 @@ class Context:
 
     def read_tap(self, what, stride=0):
         """0 softbits, 1 CIR, 2 constellation points (75 x 16 per stream), 3 null symbol (2656 samples, NCO applied),
-        5 frame results, 6 FIBs, 7 logical frames [S, MAX_SUBCH, 4, stride] and 8 superframes [S, MAX_SUBCH, stride] of the
-        last step (also after process_async)"""
+        4 TII spectra (PRS, null symbol), 5 frame results, 6 FIBs, 7 logical frames [S, MAX_SUBCH, 4, stride] and 8 superframes
+        [S, MAX_SUBCH, stride] of the last step (also after process_async), 9 TII measurements (TII_DTYPE per stream)"""
         if what == 7:
             out = np.zeros((self.n_streams, MAX_SUBCH, 4, stride), np.uint8)
         elif what == 8:
@@ -317,6 +323,8 @@ class Context:
             out = np.zeros((self.n_streams, 2656), np.complex64)
         elif what == 4:
             out = np.zeros((self.n_streams, 2, 2048), np.complex64)
+        elif what == 9:
+            out = np.zeros(self.n_streams, TII_DTYPE)
         else:
             out = np.zeros((self.n_streams, TU), np.float32)
         self._ck(self.lib.dabb_read_tap(self.h, what, _vp(out), C.c_size_t(out.nbytes)))

@@ -1,7 +1,7 @@
 /*
  * batch_decode.cpp — native batch driver over the C ABI: decodes many RAW IQ recordings at once, one stream per file, on one GPU.
  *
- *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] --out DIR file1 [file2 ...]
+ *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] --out DIR file1 [file2 ...]
  *
  * What `welle-cli -f FILE -D` does for one recording (welle-cli.cpp:215-235,612-707: dump the FIC, tune to the first audio
  * service, dump its logical frames) done for all files in lock-step: every iteration hands each stream's next window of samples
@@ -10,6 +10,9 @@
  * first audio service is selected as soon as its sub-channel is known (streams with the same protection profile share a slot of
  * the library), logical frames go to DIR/<name>.msc, Reed-Solomon statistics to DIR/<name>.rs.  Streams progress independently
  * (per-stream sample position, acquisition state, end of file).  No signal processing happens here.
+ *
+ * --tii: transmitter identification of every decoded frame, analysed on the device (dabb_options.decode_tii, tap 9); each measurement
+ * goes to DIR/<name>.tii as one line "comb pattern delay_samples error", the format of glue_test's .tii (onTIIMeasurement).
  *
  * Sample formats are the RAW-file formats of CRAWFile (input/raw_file.cpp:324-366); they are shipped as they are and converted on
  * the device.
@@ -29,7 +32,7 @@
 namespace {
 
 struct Stream {
-    std::string path, name; FILE* in = nullptr; FILE* fic = nullptr; FILE* msc = nullptr; FILE* rs = nullptr;
+    std::string path, name; FILE* in = nullptr; FILE* fic = nullptr; FILE* msc = nullptr; FILE* rs = nullptr; FILE* tii = nullptr;
     int64_t buf_start = 0, have = 0, pos = 0, acq_need = 0;      /* logical sample indices; `have` samples are buffered from buf_start */
     bool tracking = false, eof = false, done = false;
     std::unique_ptr<dabb_host::FigDb> db{new dabb_host::FigDb()};
@@ -45,7 +48,7 @@ int bytes_per_sample(int fmt) { return fmt == DABB_IQ_CF32 ? 8 : (fmt == DABB_IQ
 
 int main(int argc, char** argv)
 {
-    int fmt = DABB_IQ_CF32, device = 0; bool coarse = false; std::string out;
+    int fmt = DABB_IQ_CF32, device = 0; bool coarse = false, tii = false; std::string out;
     std::vector<std::string> files;
     for (int i = 1; i < argc; i++) {
         const std::string a = argv[i];
@@ -57,9 +60,10 @@ int main(int argc, char** argv)
         else if (a == "--device" && i + 1 < argc) device = atoi(argv[++i]);
         else if (a == "--out" && i + 1 < argc) out = argv[++i];
         else if (a == "--coarse") coarse = true;
+        else if (a == "--tii") tii = true;
         else files.push_back(a);
     }
-    if (out.empty() || files.empty()) { fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] --out DIR file...\n"); return 2; }
+    if (out.empty() || files.empty()) { fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] --out DIR file...\n"); return 2; }
 
     const int S = (int)files.size();
     const int64_t TF = DABB_TF, W = 6 * TF;                       /* per-stream window capacity in samples */
@@ -71,6 +75,11 @@ int main(int argc, char** argv)
     cfg.disable_coarse = coarse ? 0 : 1; cfg.n_subch_slots = DABB_MAX_SUBCH; cfg.max_subch_cu = 416;
     dabb_ctx* ctx = nullptr;
     if (dabb_create(&cfg, &ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return 1; }
+    if (tii) {
+        dabb_options op; memset(&op, 0, sizeof op);
+        op.disable_coarse = cfg.disable_coarse; op.decode_tii = 1;
+        if (dabb_set_options(ctx, &op) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
+    }
 
     std::vector<Stream> st((size_t)S);
     for (int s = 0; s < S; s++) {
@@ -81,7 +90,8 @@ int main(int argc, char** argv)
         z.in = fopen(z.path.c_str(), "rb");
         if (!z.in) { fprintf(stderr, "batch_decode: cannot open %s\n", z.path.c_str()); return 1; }
         z.fic = fopen((out + "/" + z.name + ".fic").c_str(), "wb"); z.msc = fopen((out + "/" + z.name + ".msc").c_str(), "wb"); z.rs = fopen((out + "/" + z.name + ".rs").c_str(), "w");
-        if (!z.fic || !z.msc || !z.rs) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
+        if (tii) z.tii = fopen((out + "/" + z.name + ".tii").c_str(), "w");
+        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
         z.acq_need = 3 * TF;
     }
     dabb_stream_reset(ctx, 0, S, 0);
@@ -91,6 +101,7 @@ int main(int argc, char** argv)
     std::vector<dabb_frame_result> res((size_t)S);
     std::vector<uint8_t> fibs((size_t)S * 12 * 32), msc((size_t)S * DABB_MAX_SUBCH * 4 * 1152), sf((size_t)S * DABB_MAX_SUBCH * 5760);
     std::vector<Profile> profiles;                               /* slot k decodes profiles[k] */
+    std::vector<dabb_tii_result> tres(tii ? (size_t)S : 0);
 
     int active = S;
     while (active > 0) {
@@ -134,12 +145,18 @@ int main(int argc, char** argv)
         io.iq = reinterpret_cast<const float*>(iq.data()); io.iq_is_host = 1; io.stride_samples = W; io.buf_start = buf_start.data(); io.buf_len = buf_len;
         io.results = res.data(); io.fibs = fibs.data(); io.msc = msc.data(); io.msc_stride = 1152; io.sf = sf.data(); io.sf_stride = 5760; io.iq_format = fmt;
         if (dabb_process(ctx, &io) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
+        if (tii && dabb_read_tap(ctx, 9, tres.data(), tres.size() * sizeof(dabb_tii_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
 
         /* 2. per-stream results */
         for (int s = 0; s < S; s++) {
             Stream& z = st[(size_t)s];
             if (z.done) continue;
             const dabb_frame_result& r = res[(size_t)s];
+            if (tii)
+                for (int i = 0; i < tres[(size_t)s].count; i++) {
+                    const auto& m = tres[(size_t)s].m[i];
+                    fprintf(z.tii, "%d %d %d %.1f\n", m.comb, m.pattern, m.delay_samples, m.error);
+                }
             if (r.status == DABB_FRAME_NEED_SAMPLES) { z.done = true; active--; continue; }      /* cannot happen for a live stream: stop it rather than spin */
             z.pos = r.next_pos;
             if (r.status == DABB_FRAME_NO_SYNC) { z.tracking = false; continue; }
@@ -190,7 +207,7 @@ int main(int argc, char** argv)
     }
     for (auto& z : st) {
         printf("%s frames=%ld fibs=%ld fib_crc_ok=%ld service=0x%X bitrate=%d logical_frames=%ld\n", z.name.c_str(), z.frames, z.fibs, z.fibs_ok, z.sid, z.bitrate, z.logical);
-        fclose(z.in); fclose(z.fic); fclose(z.msc); fclose(z.rs);
+        fclose(z.in); fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii);
     }
     dabb_destroy(ctx);
     return 0;

@@ -389,6 +389,35 @@ extern "C" int welle_b200_tii_run(const float* null_specs, const float* prs_spec
     return k;
 }
 
+/* test hook: the same analysis with the frame of every measurement; out: 5 floats per measurement (frame index 0 .. n-1, comb, pattern,
+ * delay_samples, error) in the order of the onTIIMeasurement callbacks; returns their number */
+extern "C" int welle_b200_tii_run_framed(const float* null_specs, const float* prs_specs, int n, float* out, int cap)
+{
+    dabb_host::TiiAnalyzer an; int k = 0;
+    for (int f = 0; f < n; f++)
+        an.process(reinterpret_cast<const complexf*>(null_specs) + (size_t)f * 2048, reinterpret_cast<const complexf*>(prs_specs) + (size_t)f * 2048,
+                   [&](tii_measurement_t&& m) {
+                       if (k < cap) { float* o = out + 5 * k; o[0] = (float)f; o[1] = (float)m.comb; o[2] = (float)m.pattern; o[3] = (float)m.delay_samples; o[4] = m.error; }
+                       k++; });
+    return k;
+}
+
+/* test hook: the phase-error table's container as TIIDecoder::analyse_phase uses it (tii-decoder.cpp:344-381): a
+ * std::unordered_map<float, uint64_t> filled for err = -4 .. 499 in that order, after `clears` earlier fill + clear() cycles, with
+ * value sums[err + 4]; keys_out[504]: the keys in iteration order; returns the key std::min_element picks */
+extern "C" int welle_b200_tii_map_argmin(const uint32_t* sums, int clears, int32_t* keys_out)
+{
+    std::unordered_map<float, uint64_t> m;
+    for (int c = 0; c <= clears; c++) {
+        if (c) m.clear();
+        for (int err = -4; err < 500; err++) m[(float)err] += c == clears ? sums[err + 4] : 0;
+    }
+    int i = 0;
+    for (const auto& kv : m) keys_out[i++] = (int32_t)kv.first;
+    const auto best = std::min_element(m.begin(), m.end(), [](const std::pair<const float, uint64_t>& a, const std::pair<const float, uint64_t>& b) { return a.second < b.second; });
+    return (int)best->first;
+}
+
 /* test hook: feeds n FIBs (32 bytes each) to a fresh service database and writes its text dump (callbacks first) */
 extern "C" int welle_b200_figdb_dump(const uint8_t* fibs, int n, char* out, int cap)
 {
