@@ -134,6 +134,14 @@ typedef struct {
     int32_t eep_level;    /* 1..4 */
     int32_t dabplus;      /* 1 = DAB+ (RS + Fire code + AU CRC), 0 = DAB MP2 (logical frames only) */
 } dabb_subchannel;
+/* Streams in one slot are independent: each may use its own sub-channel, bitrate, protection profile and DAB/DAB+, and a call that
+ * selects or removes some streams leaves the decoding of every other stream of the slot byte for byte as it was (the named streams
+ * restart their time de-interleaver and superframe search).  A context holds up to DABB_MAX_PROFILES distinct protection profiles
+ * (bitrate + UEP level or EEP profile/level), counted over all slots from its creation on; a select call that would add one more
+ * returns DABB_E_UNSUPPORTED and changes nothing.  Step outputs: a stream's logical frames are 3*bitrate bytes and its superframes
+ * 15*bitrate bytes of its own bitrate, so msc_stride / sf_stride must cover the largest of them among the streams enabled in any
+ * slot; bytes behind a stream's own length, and the rows of streams not enabled in a slot, are left as the caller had them. */
+enum { DABB_MAX_PROFILES = 64 };
 int dabb_select_subchannel(dabb_ctx* ctx, int32_t first_stream, int32_t count, int32_t slot, const dabb_subchannel* sc);
 int dabb_remove_subchannel(dabb_ctx* ctx, int32_t first_stream, int32_t count, int32_t slot);
 

@@ -95,7 +95,7 @@ struct dabb_ctx {
     // combinations and their phase-error sums, the step's analyses, the tie-order tables and the step's records (tap 9)
     DevBuf<float2> d_tii_null; DevBuf<dabb_tii::StreamHdr> d_tii_hdr; DevBuf<dabb_tii::Job> d_tii_jobs; DevBuf<int32_t> d_tii_njobs;
     DevBuf<uint32_t> d_tii_sums; DevBuf<uint16_t> d_tii_rank; DevBuf<dabb_tii_result> d_tii_res;
-    bool persistent = false; DevBuf<unsigned int> d_work; TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0; int flen_max = 0;
+    bool persistent = false; DevBuf<unsigned int> d_work; TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0;
     DevBuf<unsigned long long> d_trace_rec; DevBuf<unsigned int> d_trace_count;      // what `trace` points into
     std::string err; int64_t launches = 0; int osc_mismatches = -1; int osc_patched = 0; std::vector<float2> h_osc;
     HostTables* host = nullptr; DevTables dev{};
@@ -105,11 +105,22 @@ struct dabb_ctx {
     DevBuf<int32_t> d_active, d_index; DevBuf<float> d_cir, d_cir_work; int search_generic = 0; int vit_split = 0; DevBuf<float2> d_r1, d_null; DevBuf<int32_t> d_snr; DevBuf<float2> d_fc; DevBuf<float> d_lvl;
     DevBuf<int8_t> d_soft; DevBuf<uint2> d_fic_steptab; DevBuf<uint32_t> d_fic_stage_off; DevBuf<uint2> d_dec; DevBuf<uint8_t> d_fibs; DevBuf<int32_t> d_crc;
     DevBuf<dabb_frame_result> d_results;
-    // per slot: everything sized by the slot's code geometry, so that a new geometry starts from an empty Slot
+    // the protection-profile table: one entry per distinct ProtProfile a select call has met, built the first time it is selected and
+    // kept until dabb_destroy (MscSlotState::profile indexes it); d_profiles holds their device tables for the grouped Viterbi launch
+    struct Profile {
+        ProtProfile prof{}; int nsteps = 0, nbits = 0, flen = 0, flen_pad = 0;
+        DevBuf<uint2> d_steptab; DevBuf<uint32_t> d_stage_off, d_prbs_words;
+    };
+    std::vector<Profile> profiles; DevBuf<VitProfile> d_profiles;
+    // per slot: the buffers of the streams that decode a sub-channel in it.  Rows of d_logical / d_window / d_sf are flen_pad bytes
+    // (x 1 / 5 / 5), the largest flen_pad the slot has held, so that a stream keeps its row when another stream's geometry changes;
+    // flen is the largest logical frame among the slot's enabled streams (0: none).  The MSC Viterbi launch runs the grouped schedule
+    // d_groups / d_cw_list (vit_groups.cuh), rebuilt by every select and remove call.
     struct Slot {
-        bool configured = false; ProtProfile prof{}; int nsteps = 0, nbits = 0, frag_pitch = 0, flen = 0, flen_pad = 0;
-        DevBuf<uint2> d_steptab; DevBuf<uint32_t> d_stage_off, d_prbs_words; DevBuf<int8_t> d_frag; DevBuf<int32_t> d_valid;
+        bool configured = false; int frag_pitch = 0, flen = 0, flen_pad = 0, n_groups = 0;
+        DevBuf<int8_t> d_frag; DevBuf<int32_t> d_valid;
         DevBuf<uint8_t> d_logical; DevBuf<uint2> d_dec; DevBuf<uint8_t> d_window, d_sf; DevBuf<int32_t> d_info;
+        DevBuf<VitGroup> d_groups; DevBuf<int32_t> d_cw_list;
     } slot[DABB_MAX_SUBCH];
     DevBuf<int8_t> d_ring[DABB_MAX_SUBCH];     // per slot: the time de-interleaver's history, kept when the slot's geometry changes
     DevBuf<uint32_t> d_fic_prbs_words;
@@ -123,7 +134,8 @@ struct dabb_ctx {
     struct Pending {
         cudaEvent_t done = nullptr; StepOut out{};
         HostBuf<dabb_frame_result> h_res; HostBuf<uint8_t> h_fibs, h_logical, h_superframe;
-        int flen[DABB_MAX_SUBCH] = {0, 0, 0, 0}, flen_pad[DABB_MAX_SUBCH] = {0, 0, 0, 0}; size_t msc_off[DABB_MAX_SUBCH] = {0, 0, 0, 0}, sf_off[DABB_MAX_SUBCH] = {0, 0, 0, 0};
+        int flen_pad[DABB_MAX_SUBCH] = {0, 0, 0, 0}; size_t msc_off[DABB_MAX_SUBCH] = {0, 0, 0, 0}, sf_off[DABB_MAX_SUBCH] = {0, 0, 0, 0};    // flen_pad 0: slot not configured
+        std::vector<int32_t> flen;      // [slot][stream] the stream's logical frame length when the step was enqueued (0: nothing to deliver)
     } pend[2], pend_sync;     // the two dabb_submit slots; dabb_process and taps 7 / 8, which never leave a step outstanding
     int pend_head = 0, pend_count = 0; int64_t submits = 0;
     int groups = 1; int fc_pitch = 1; int tail_frames = 0; int tail_groups = 5; int nco_fast = 0;
@@ -501,12 +513,17 @@ int prepare_pending(dabb_ctx* ctx, dabb_ctx::Pending& p)
     if (!p.h_res && (rc = alloc(ctx, p.h_res, S))) return rc;
     if (!p.h_fibs && (rc = alloc(ctx, p.h_fibs, (size_t)S * 12 * 32))) return rc;
     size_t msc = 0, sf = 0;
+    p.flen.assign((size_t)ctx->n_slots * S, 0);
     for (int k = 0; k < ctx->n_slots; k++) {
         const auto& sl = ctx->slot[k];
-        p.flen[k] = sl.configured ? sl.flen : 0; p.flen_pad[k] = sl.flen_pad;
+        p.flen_pad[k] = sl.configured ? sl.flen_pad : 0;
         if (!sl.configured) continue;
         p.msc_off[k] = msc; p.sf_off[k] = sf;
         msc += (size_t)S * 4 * sl.flen_pad; sf += (size_t)S * 5 * sl.flen_pad;
+        for (int s = 0; s < S; s++) {       // the geometry the step runs with: a select call before dabb_collect does not change it
+            const MscSlotState& m = ctx->h_slots[(size_t)s * ctx->n_slots + k];
+            p.flen[(size_t)k * S + s] = m.enabled ? 3 * m.bitrate : 0;
+        }
     }
     if (msc > p.h_logical.size() && (rc = alloc(ctx, p.h_logical, msc))) return rc;
     if (sf > p.h_superframe.size() && (rc = alloc(ctx, p.h_superframe, sf))) return rc;
@@ -521,7 +538,7 @@ int enqueue_readback(dabb_ctx* ctx, dabb_ctx::Pending& p, const StepOut& o)
     if (o.results) CK(cudaMemcpyAsync(p.h_res, ctx->d_results, sizeof(dabb_frame_result) * S, cudaMemcpyDeviceToHost, B));
     if (o.fibs) CK(cudaMemcpyAsync(p.h_fibs, ctx->d_fibs, (size_t)S * 12 * 32, cudaMemcpyDeviceToHost, B));
     for (int k = 0; k < ctx->n_slots; k++) {
-        if (!p.flen[k]) continue;
+        if (!p.flen_pad[k]) continue;
         const auto& sl = ctx->slot[k];
         if (o.msc) CK(cudaMemcpyAsync(p.h_logical + p.msc_off[k], sl.d_logical, (size_t)S * 4 * p.flen_pad[k], cudaMemcpyDeviceToHost, B));
         if (o.sf) CK(cudaMemcpyAsync(p.h_superframe + p.sf_off[k], sl.d_sf, (size_t)S * 5 * p.flen_pad[k], cudaMemcpyDeviceToHost, B));
@@ -539,15 +556,88 @@ int deliver(dabb_ctx* ctx, dabb_ctx::Pending& p)
     if (o.results) memcpy(o.results, p.h_res, sizeof(dabb_frame_result) * S);
     if (o.fibs) memcpy(o.fibs, p.h_fibs, (size_t)S * 12 * 32);
     for (int k = 0; k < ctx->n_slots; k++) {
-        const size_t flen = p.flen[k], fp = p.flen_pad[k];
-        if (!flen) continue;
-        if (o.msc)       // pinned rows [S*4][fp] -> caller [S][MAX_SUBCH][4][msc_stride]
-            for (int s = 0; s < S; s++) for (int c = 0; c < 4; c++)
-                memcpy(o.msc + (((size_t)s * DABB_MAX_SUBCH + k) * 4 + c) * o.msc_stride, p.h_logical + p.msc_off[k] + ((size_t)s * 4 + c) * fp, flen);
-        if (o.sf)
-            for (int s = 0; s < S; s++) memcpy(o.sf + ((size_t)s * DABB_MAX_SUBCH + k) * o.sf_stride, p.h_superframe + p.sf_off[k] + (size_t)s * 5 * fp, 5 * flen);
+        const size_t fp = p.flen_pad[k];
+        if (!fp) continue;
+        for (int s = 0; s < S; s++) {    // each stream's own frame length; streams not enabled in the slot keep the caller's bytes
+            const size_t flen = p.flen[(size_t)k * S + s];
+            if (!flen) continue;
+            if (o.msc)   // pinned rows [S*4][fp] -> caller [S][MAX_SUBCH][4][msc_stride]
+                for (int c = 0; c < 4; c++)
+                    memcpy(o.msc + (((size_t)s * DABB_MAX_SUBCH + k) * 4 + c) * o.msc_stride, p.h_logical + p.msc_off[k] + ((size_t)s * 4 + c) * fp, flen);
+            if (o.sf) memcpy(o.sf + ((size_t)s * DABB_MAX_SUBCH + k) * o.sf_stride, p.h_superframe + p.sf_off[k] + (size_t)s * 5 * fp, 5 * flen);
+        }
     }
     return DABB_OK;
+}
+
+// ---- sub-channel slots ----------------------------------------------------------------------------------------------------------
+// a new entry of the protection-profile table: the de-puncturing expansion tables and dispersal words of its code geometry
+int add_profile(dabb_ctx* ctx, const ProtProfile& prof)
+{
+    dabb_ctx::Profile pf;
+    pf.prof = prof; pf.nbits = 24 * prof.bitrate; pf.nsteps = pf.nbits + 6; pf.flen = 3 * prof.bitrate; pf.flen_pad = (pf.flen + 15) & ~15;
+    std::vector<int16_t> map((size_t)pf.nsteps * 4);
+    build_msc_map(*ctx->host, prof, map.data());
+    std::vector<uint2> steps; std::vector<uint32_t> soff;
+    build_vit_tables_u2(map.data(), pf.nsteps, steps, soff);
+    std::vector<uint32_t> w; pack_prbs_words(ctx->host->prbs, pf.nbits, w);
+    int rc;
+    if ((rc = dalloc(ctx, pf.d_steptab, steps.size(), false)) || (rc = dalloc(ctx, pf.d_stage_off, soff.size(), false)) || (rc = dalloc(ctx, pf.d_prbs_words, w.size(), false))) return rc;
+    VitProfile e{pf.d_steptab, pf.d_stage_off, pf.d_prbs_words, pf.nsteps, pf.nbits};
+    CK(cudaMemcpyAsync(pf.d_steptab, steps.data(), steps.size() * sizeof(uint2), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(pf.d_stage_off, soff.data(), soff.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(pf.d_prbs_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_profiles + ctx->profiles.size(), &e, sizeof e, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->profiles.push_back(std::move(pf));
+    return DABB_OK;
+}
+
+// b: rows of old_pitch bytes -> rows of new_pitch bytes (> old_pitch), contents kept, the new bytes zero
+int repitch(dabb_ctx* ctx, DevBuf<uint8_t>& b, size_t rows, size_t old_pitch, size_t new_pitch)
+{
+    DevBuf<uint8_t> nb;
+    int rc;
+    if ((rc = dalloc(ctx, nb, rows * new_pitch))) return rc;
+    CK(cudaMemcpy2DAsync(nb, new_pitch, b, old_pitch, old_pitch, rows, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    b = std::move(nb);
+    return DABB_OK;
+}
+
+// streams [first, first + count) of `slot` take state v (v.enabled = 0: removed).  The slot's grouped Viterbi schedule, its decision
+// buffer and its largest frame length follow the new membership; the new buffers are allocated and filled before any is replaced, so
+// that a failed allocation leaves the slot as it was.  Every other stream's state and buffers are untouched.  (The caller has run
+// sync_all: nothing on the device uses the buffers replaced here.)
+int set_slot_streams(dabb_ctx* ctx, int slot, int first, int count, const MscSlotState& v)
+{
+    const int S = ctx->S, ns = ctx->n_slots;
+    auto& sl = ctx->slot[slot];
+    int rc;
+    if (sl.configured) {
+        std::vector<int32_t> prof_of((size_t)S), nsteps(ctx->profiles.size());
+        int flen = 0;
+        for (int s = 0; s < S; s++) {
+            const MscSlotState& m = (s >= first && s < first + count) ? v : ctx->h_slots[(size_t)s * ns + slot];
+            prof_of[(size_t)s] = m.enabled ? m.profile : -1;
+            if (m.enabled) flen = std::max(flen, 3 * m.bitrate);
+        }
+        for (size_t i = 0; i < ctx->profiles.size(); i++) nsteps[i] = ctx->profiles[i].nsteps;
+        VitSchedule sch;
+        build_vit_schedule(prof_of.data(), S, nsteps.data(), (int)nsteps.size(), sch);
+        DevBuf<uint2> dec; DevBuf<VitGroup> groups; DevBuf<int32_t> list;
+        if (((size_t)sch.dec_words > sl.d_dec.size() && (rc = alloc(ctx, dec, (size_t)sch.dec_words))) ||
+            (rc = alloc(ctx, groups, sch.groups.size())) || (rc = alloc(ctx, list, sch.list.size())))
+            return rc;
+        CK(cudaMemcpyAsync(groups, sch.groups.data(), sch.groups.size() * sizeof(VitGroup), cudaMemcpyHostToDevice, ctx->stream));
+        if (!sch.list.empty()) CK(cudaMemcpyAsync(list, sch.list.data(), sch.list.size() * sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        if (dec) sl.d_dec = std::move(dec);
+        sl.d_groups = std::move(groups); sl.d_cw_list = std::move(list); sl.n_groups = (int)sch.groups.size(); sl.flen = flen;
+    }
+    set_slot_kernel<<<(count + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_slots, ns, slot, first, count, v);
+    for (int i = first; i < first + count; i++) ctx->h_slots[(size_t)i * ns + slot] = v;
+    { int rc_ = check_launch(ctx, "set_slot_kernel"); cudaStreamSynchronize(ctx->stream); return rc_; }
 }
 
 } // namespace
@@ -689,6 +779,8 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     if (ctx->keep_taps && ((rc = dalloc(ctx, ctx->d_cir, (size_t)S * TU)) || (rc = dalloc(ctx, ctx->d_r1, (size_t)S * 75 * 1536)) || (rc = dalloc(ctx, ctx->d_null, (size_t)S * TNULL)))) return fail(rc);
     if ((rc = dalloc(ctx, ctx->d_dec, vit_dec_bytes(S * 4, 774) / sizeof(uint2), false)) || (rc = dalloc(ctx, ctx->d_dec_fic, vit_dec_bytes(S * 4, 774) / sizeof(uint2), false))) return fail(rc);
     ctx->h_slots.assign((size_t)S * ctx->n_slots, MscSlotState{});
+    ctx->profiles.reserve(DABB_MAX_PROFILES);
+    if ((rc = dalloc(ctx, ctx->d_profiles, DABB_MAX_PROFILES))) return fail(rc);
     // info arrays of unconfigured slots are never read (finalize skips disabled slots)
     if ((rc = prepare_pending(ctx, ctx->pend_sync))) return fail(rc);
     {
@@ -768,42 +860,36 @@ int dabb_select_subchannel(dabb_ctx* ctx, int32_t first, int32_t count, int32_t 
     if (sc->length_cu < 1 || sc->length_cu > ctx->max_cu || sc->start_cu < 0 || sc->start_cu + sc->length_cu > 864) { ctx->err = "sub-channel does not fit (raise dabb_config.max_subch_cu)"; return DABB_E_ARG; }
     if (prof.in_bits > sc->length_cu * 64) { ctx->err = "protection profile needs more bits than the sub-channel holds"; return DABB_E_ARG; }
     if (sc->dabplus && sc->bitrate / 8 > 64) { ctx->err = "DAB+ sub-channels above 512 kbit/s are not supported"; return DABB_E_UNSUPPORTED; }
+    int pi = -1;
+    for (size_t i = 0; i < ctx->profiles.size(); i++) if (!memcmp(&ctx->profiles[i].prof, &prof, sizeof prof)) pi = (int)i;
+    if (pi < 0 && ctx->profiles.size() >= (size_t)DABB_MAX_PROFILES) {
+        ctx->err = "more than " + std::to_string(DABB_MAX_PROFILES) + " distinct protection profiles in one context"; return DABB_E_UNSUPPORTED;
+    }
+    int rc = 0;
+    if (pi < 0 && (rc = add_profile(ctx, prof))) return rc;
+    if (pi < 0) pi = (int)ctx->profiles.size() - 1;
+    const auto& pf = ctx->profiles[(size_t)pi];
     auto& sl = ctx->slot[slot];
     const int S = ctx->S;
-    int rc = 0;
-    if (sl.configured && (memcmp(&sl.prof, &prof, sizeof prof) != 0)) {
-        // a slot decodes one code geometry for all its streams in one launch
-        bool others = false;
-        for (int i = 0; i < S; i++) if ((i < first || i >= first + count) && ctx->h_slots[(size_t)i * ctx->n_slots + slot].enabled) others = true;
-        if (others) { ctx->err = "streams sharing a slot must use the same bitrate/protection; use another slot"; return DABB_E_UNSUPPORTED; }
-        // the slot changes its code geometry: give back the buffers sized for the old one (all streams are idle: sync_all above)
-        sl = dabb_ctx::Slot{};
-    }
-    if (!sl.configured) {
-        sl.prof = prof; sl.nbits = 24 * prof.bitrate; sl.nsteps = sl.nbits + 6; sl.frag_pitch = ctx->ring_pitch; sl.flen = 3 * prof.bitrate; sl.flen_pad = (sl.flen + 15) & ~15;
-        std::vector<int16_t> map((size_t)sl.nsteps * 4);
-        build_msc_map(*ctx->host, prof, map.data());
-        std::vector<uint2> steps; std::vector<uint32_t> soff;
-        build_vit_tables_u2(map.data(), sl.nsteps, steps, soff);
-        std::vector<uint32_t> w; pack_prbs_words(ctx->host->prbs, sl.nbits, w);
-        if ((rc = dalloc(ctx, sl.d_steptab, steps.size())) || (rc = dalloc(ctx, sl.d_stage_off, soff.size())) || (rc = dalloc(ctx, sl.d_prbs_words, w.size())) ||
-            (rc = dalloc(ctx, sl.d_frag, (size_t)S * 4 * sl.frag_pitch + VIT_FRAG_SLACK)) ||
+    const bool fresh = !sl.configured;
+    if (fresh) {
+        sl.frag_pitch = ctx->ring_pitch; sl.flen_pad = pf.flen_pad;
+        if ((rc = dalloc(ctx, sl.d_frag, (size_t)S * 4 * sl.frag_pitch + VIT_FRAG_SLACK)) ||
             (rc = dalloc(ctx, sl.d_valid, (size_t)S * 4)) || (rc = dalloc(ctx, sl.d_logical, (size_t)S * 4 * sl.flen_pad)) ||
             (rc = dalloc(ctx, sl.d_window, (size_t)S * 5 * sl.flen_pad)) || (rc = dalloc(ctx, sl.d_sf, (size_t)S * 5 * sl.flen_pad)) ||
-            (rc = dalloc(ctx, sl.d_info, (size_t)S * 16)) || (rc = dalloc(ctx, sl.d_dec, vit_dec_bytes(S * 4, sl.nsteps) / sizeof(uint2), false)))
-            return rc;
-        if (!ctx->d_ring[slot] && (rc = dalloc(ctx, ctx->d_ring[slot], (size_t)S * MSC_RING * ctx->ring_pitch))) return rc;
-        CK(cudaMemcpyAsync(sl.d_steptab, steps.data(), steps.size() * sizeof(uint2), cudaMemcpyHostToDevice, ctx->stream));
-        CK(cudaMemcpyAsync(sl.d_stage_off, soff.data(), soff.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-        CK(cudaMemcpyAsync(sl.d_prbs_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
+            (rc = dalloc(ctx, sl.d_info, (size_t)S * 16)))
+            { sl = dabb_ctx::Slot{}; return rc; }
+        if (!ctx->d_ring[slot] && (rc = dalloc(ctx, ctx->d_ring[slot], (size_t)S * MSC_RING * ctx->ring_pitch))) { sl = dabb_ctx::Slot{}; return rc; }
         sl.configured = true;
-        if (sl.flen > ctx->flen_max) ctx->flen_max = sl.flen;
+    } else if (pf.flen_pad > sl.flen_pad) {
+        // wider rows: every stream's logical frames, superframe window and last superframe move into the new layout unchanged
+        const size_t o = (size_t)sl.flen_pad, n = (size_t)pf.flen_pad;
+        if ((rc = repitch(ctx, sl.d_logical, (size_t)S * 4, o, n)) || (rc = repitch(ctx, sl.d_window, S, 5 * o, 5 * n)) || (rc = repitch(ctx, sl.d_sf, S, 5 * o, 5 * n))) return rc;
+        sl.flen_pad = pf.flen_pad;
     }
-    MscSlotState v{}; v.enabled = 1; v.start_cu = sc->start_cu; v.frag = sc->length_cu * 64; v.bitrate = sc->bitrate; v.dabplus = sc->dabplus; v.cif_count = 0; v.sf_frame_count = 0;
-    set_slot_kernel<<<(count + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_slots, ctx->n_slots, slot, first, count, v);
-    for (int i = first; i < first + count; i++) ctx->h_slots[(size_t)i * ctx->n_slots + slot] = v;
-    { int rc_ = check_launch(ctx, "set_slot_kernel"); cudaStreamSynchronize(ctx->stream); return rc_; }
+    MscSlotState v{}; v.enabled = 1; v.start_cu = sc->start_cu; v.frag = sc->length_cu * 64; v.bitrate = sc->bitrate; v.dabplus = sc->dabplus; v.profile = pi; v.cif_count = 0; v.sf_frame_count = 0;
+    if ((rc = set_slot_streams(ctx, slot, first, count, v))) { if (fresh) sl = dabb_ctx::Slot{}; return rc; }
+    return DABB_OK;
 }
 
 int dabb_remove_subchannel(dabb_ctx* ctx, int32_t first, int32_t count, int32_t slot)
@@ -811,10 +897,7 @@ int dabb_remove_subchannel(dabb_ctx* ctx, int32_t first, int32_t count, int32_t 
     if (!ctx || first < 0 || count < 1 || first + count > ctx->S || slot < 0 || slot >= ctx->n_slots) return DABB_E_ARG;
     cudaSetDevice(ctx->device);
     sync_all(ctx);
-    MscSlotState v{};
-    set_slot_kernel<<<(count + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_slots, ctx->n_slots, slot, first, count, v);
-    for (int i = first; i < first + count; i++) ctx->h_slots[(size_t)i * ctx->n_slots + slot] = v;
-    { int rc_ = check_launch(ctx, "set_slot_kernel"); cudaStreamSynchronize(ctx->stream); return rc_; }
+    return set_slot_streams(ctx, slot, first, count, MscSlotState{});
 }
 
 
@@ -980,9 +1063,10 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         pp.frag_out = sl.d_frag; pp.frag_pitch = sl.frag_pitch; pp.valid = sl.d_valid;
         launch_msc_gather(pp, S, B);
         if ((rc = check_launch(ctx, "msc_gather_kernel"))) return rc;
-        ViterbiParams vp{}; vp.frag = sl.d_frag; vp.cw_div = 1; vp.outer_stride = sl.frag_pitch; vp.inner_stride = 0; vp.steptab = sl.d_steptab; vp.stage_off = sl.d_stage_off;
-        vp.n_cw = S * 4; vp.nsteps = sl.nsteps; vp.nbits = sl.nbits; vp.dec = sl.d_dec;
-        vp.out = sl.d_logical; vp.out_stride = sl.flen_pad; vp.prbs_words = sl.d_prbs_words; vp.valid = sl.d_valid;
+        // one launch for all the slot's profiles: each CTA decodes codewords of one profile (vit_groups.cuh)
+        ViterbiParams vp{}; vp.frag = sl.d_frag; vp.cw_div = 1; vp.outer_stride = sl.frag_pitch; vp.inner_stride = 0;
+        vp.groups = sl.d_groups; vp.cw_list = sl.d_cw_list; vp.profiles = ctx->d_profiles; vp.n_groups = sl.n_groups;
+        vp.n_cw = S * 4; vp.dec = sl.d_dec; vp.out = sl.d_logical; vp.out_stride = sl.flen_pad; vp.valid = sl.d_valid;
         vp.trace = ctx->trace; vp.trace_kind = 3; vp.split = ctx->vit_split;
         launch_viterbi(vp, B, ctx->vit_stages_now);
         if ((rc = check_launch(ctx, "viterbi_kernel(MSC)"))) return rc;

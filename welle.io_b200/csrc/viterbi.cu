@@ -12,8 +12,8 @@
 // the PUNCTURED softbits (FIC: straight from the OFDM kernel's output; MSC: the gathered fragment): per 24 trellis steps every
 // thread stages the 16-byte aligned 128 bytes that hold its next <= 96 softbits into shared memory with cp.async.bulk (TMA,
 // completion on an mbarrier, 3-stage ring) and expands them itself - the puncturing pattern is the same for every codeword of a
-// launch, so the byte selector / mask / window-advance flag of each step come from one small table (build_vit_tables) and the
-// expansion of a step is PRMT + LOP3 + IADD.  Decision words go to HBM/L2 as 8 bytes per step per codeword and are read back by
+// CTA (of the launch, or of the CTA's profile in a grouped MSC launch, vit_groups.cuh), so the byte selector / mask /
+// window-advance flag of each step come from one small table (build_vit_tables) and the expansion of a step is PRMT + LOP3 + IADD.  Decision words go to HBM/L2 as 8 bytes per step per codeword and are read back by
 // the same thread for the traceback.  Issue-slot bound (integer ACS).
 #include "common.cuh"
 #include "viterbi_core.cuh"
@@ -143,16 +143,48 @@ __device__ __forceinline__ void cp_async16(void* dst_smem, const void* src_gmem)
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
+// What one CTA decodes.  Ungrouped: codewords 128 b .. 128 b + 127 (below n_cw) with the launch's tables.  Grouped: the codewords and
+// the profile of descriptor b (vit_groups.cuh); every CTA still has one profile, so all the warp-uniform structure below holds.
+struct VitJob {
+    const uint2* steptab; const uint32_t* stage_off;
+    int nsteps;
+    int cw; bool have;               // this thread's codeword (a valid index even where have is false)
+    uint2* dec;                      // this thread's first decision word
+    const VitProfile* prof;          // grouped: the CTA's profile (its energy-dispersal words are read for the traceback)
+};
+template <bool GROUPED>
+__device__ __forceinline__ bool viterbi_job(const ViterbiParams& p, const int block, const int t, VitJob& j)
+{
+    if constexpr (GROUPED) {
+        const VitGroup g = p.groups[block];
+        if (g.count == 0) return false;                              // a slot without enabled streams
+        j.prof = p.profiles + g.profile;
+        j.steptab = j.prof->steptab; j.stage_off = j.prof->stage_off; j.nsteps = j.prof->nsteps;
+        j.have = t < g.count;
+        j.cw = __ldg(p.cw_list + g.first + (j.have ? t : 0));
+        j.dec = p.dec + g.dec_off + t;
+    } else {
+        j.steptab = p.steptab; j.stage_off = p.stage_off; j.nsteps = p.nsteps; j.prof = nullptr;
+        const int cw = block * VIT_THREADS + t;
+        j.have = cw < p.n_cw;
+        j.cw = j.have ? cw : 0;
+        j.dec = p.dec + (int64_t)block * p.nsteps * VIT_THREADS + t;
+    }
+    return true;
+}
+// the output length and dispersal words of the job's codewords, read after the forward pass
+template <bool GROUPED> __device__ __forceinline__ int vit_job_nbits(const ViterbiParams& p, const VitJob& j) { return GROUPED ? j.prof->nbits : p.nbits; }
+template <bool GROUPED> __device__ __forceinline__ const uint32_t* vit_job_prbs(const ViterbiParams& p, const VitJob& j) { return GROUPED ? j.prof->prbs_words : p.prbs_words; }
+
 // traceback of one codeword (vit_traceback24): 96 steps (nbits is a multiple of 96) give three output words; the decision words are read
 // in batches of 24 independent loads (their addresses do not depend on the path).  dec: this thread's first decision word (stride
 // VIT_THREADS per step)
-__device__ __forceinline__ void viterbi_traceback(const ViterbiParams& p, const int cw, const uint2* dec)
+__device__ __forceinline__ void viterbi_traceback(const ViterbiParams& p, const int cw, const uint2* dec, const int nbits, const uint32_t* prbs)
 {
     if (p.valid && !p.valid[cw]) return;
     uint32_t state = 0;
     uint32_t* out = reinterpret_cast<uint32_t*>(p.out + (int64_t)cw * p.out_stride);
-    const uint32_t* prbs = p.prbs_words;
-    for (int tb = p.nbits - 96; tb >= 0; tb -= 96) {
+    for (int tb = nbits - 96; tb >= 0; tb -= 96) {
         uint32_t acc[3] = {0, 0, 0};
         vit_u2 d[24];
         // the decision words of a 32 768-codeword launch (0.6 GB) have mostly left the L2 by the time the traceback wants them: the batch
@@ -179,25 +211,27 @@ __device__ __forceinline__ void viterbi_traceback(const ViterbiParams& p, const 
 // The stage's expansion entries (the same for all codewords) are copied once per WARP by twelve of its lanes into a warp-private
 // area and read after a __syncwarp: no __syncthreads in the loop at all.
 // VIT_STAGES = 3: stand-alone launches (deep prefetch).  VIT_STAGES = 1: 19 KB of shared memory (co-residency experiment).
-template <int VIT_STAGES>
+template <int VIT_STAGES, bool GROUPED>
 __device__ __forceinline__ void viterbi_cta(const ViterbiParams& p, const int block)
 {
     extern __shared__ __align__(16) unsigned char smraw[];
     VitSmemT<VIT_STAGES>& sm = *reinterpret_cast<VitSmemT<VIT_STAGES>*>(smraw);
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const unsigned long long trace_t0 = p.trace.rec ? trace_now() : 0ull;
-    const int cw = block * VIT_THREADS + t;
-    const bool have = cw < p.n_cw;
-    const int groups = p.nsteps / 6;                 // 6 steps per group, 4 groups per stage
+    VitJob job;
+    if (!viterbi_job<GROUPED>(p, block, t, job)) return;
+    const int cw = job.cw;
+    const bool have = job.have;
+    const int groups = job.nsteps / 6;               // 6 steps per group, 4 groups per stage
     const int nstages = (groups + 3) / 4;
-    const int cwc = have ? cw : 0;
-    const unsigned char* frag = reinterpret_cast<const unsigned char*>(p.frag) + (int64_t)(cwc / p.cw_div) * p.outer_stride + (int64_t)(cwc % p.cw_div) * p.inner_stride;
-    const unsigned char* tabsrc = reinterpret_cast<const unsigned char*>(p.steptab);
+    const uint32_t* stage_off = job.stage_off;
+    const unsigned char* frag = reinterpret_cast<const unsigned char*>(p.frag) + (int64_t)(cw / p.cw_div) * p.outer_stride + (int64_t)(cw % p.cw_div) * p.inner_stride;
+    const unsigned char* tabsrc = reinterpret_cast<const unsigned char*>(job.steptab);
 
     // stage s needs the softbits [stage_off[s], stage_off[s+1]) of the fragment; always one commit group per call
     auto issue = [&](int s, int buf) {
         if (s < nstages) {
-            const unsigned char* src = frag + (__ldg(p.stage_off + s) & ~15u);
+            const unsigned char* src = frag + (__ldg(stage_off + s) & ~15u);
             unsigned char* dst = &sm.stage[buf][t * VIT_ROW_PITCH];
 #pragma unroll
             for (int k = 0; k < 8; k++) cp_async16(dst + 16 * k, src + 16 * k);
@@ -209,7 +243,7 @@ __device__ __forceinline__ void viterbi_cta(const ViterbiParams& p, const int bl
 
     uint32_t Q[32];
     vit_init(Q);
-    uint2* dec = p.dec + (int64_t)block * p.nsteps * VIT_THREADS + t;
+    uint2* dec = job.dec;
 
     for (int s = 0; s < nstages; s++) {
         const int buf = s % VIT_STAGES;
@@ -219,7 +253,7 @@ __device__ __forceinline__ void viterbi_cta(const ViterbiParams& p, const int bl
         // 8-byte window (w0, w1) over the thread's row; everything about the window but its content is the same for all threads
         const uint32_t* my = reinterpret_cast<const uint32_t*>(&sm.stage[buf][t * VIT_ROW_PITCH]);
         const uint2* tab = reinterpret_cast<const uint2*>(&sm.tab[buf][warp][0]);
-        int nx = (int)((__ldg(p.stage_off + s) & 15u) >> 2);
+        int nx = (int)((__ldg(stage_off + s) & 15u) >> 2);
         uint32_t w0 = my[nx], w1 = my[nx + 1];
         nx += 2;
         // the expansion of group g + 1 (table loads, window loads) is issued before the add-compare-select of group g: independent work
@@ -256,24 +290,26 @@ __device__ __forceinline__ void viterbi_cta(const ViterbiParams& p, const int bl
     if (p.trace.rec && t == 0) trace_put(p.trace, p.trace_kind, trace_t0);       // forward pass of thread 0 done
     if (p.split) return;                 // the traceback runs as its own launch (viterbi_tb_kernel)
     if (!have) return;
-    viterbi_traceback(p, cw, dec);
+    viterbi_traceback(p, cw, dec, vit_job_nbits<GROUPED>(p, job), vit_job_prbs<GROUPED>(p, job));
     if (p.trace.rec && t == 0) trace_put(p.trace, p.trace_kind + 10u, trace_t0);  // ... and its traceback
 }
 
-template <int VIT_STAGES>
+// GROUPED: the MSC launch of a sub-channel slot (ViterbiParams::groups); the FIC and the stage-level entry points use the plain form
+template <int VIT_STAGES, bool GROUPED>
 __global__ void __launch_bounds__(VIT_THREADS, VIT_MIN_CTAS)
-viterbi_kernel(ViterbiParams p) { viterbi_cta<VIT_STAGES>(p, blockIdx.x); }
+viterbi_kernel(ViterbiParams p) { viterbi_cta<VIT_STAGES, GROUPED>(p, blockIdx.x); }
 
 // the traceback as its own launch (ViterbiParams::split, DABB_VIT_SPLIT=1): a serial walk per codeword bound by the latency of its
 // decision loads, without shared memory, so that the SMs can take the next kernels' CTAs beside it - which the fused kernel's 57 KB
 // CTAs keep out while they walk.  Measured: no gain (4.45 vs 4.43 ms per step), so the fused form stays the default.
+template <bool GROUPED>
 __global__ void __launch_bounds__(VIT_THREADS, 4)
 viterbi_tb_kernel(ViterbiParams p)
 {
     const unsigned long long trace_t0 = p.trace.rec ? trace_now() : 0ull;
-    const int cw = blockIdx.x * VIT_THREADS + threadIdx.x;
-    if (cw >= p.n_cw) return;
-    viterbi_traceback(p, cw, p.dec + (int64_t)blockIdx.x * p.nsteps * VIT_THREADS + threadIdx.x);
+    VitJob job;
+    if (!viterbi_job<GROUPED>(p, blockIdx.x, threadIdx.x, job) || !job.have) return;
+    viterbi_traceback(p, job.cw, job.dec, vit_job_nbits<GROUPED>(p, job), vit_job_prbs<GROUPED>(p, job));
     if (p.trace.rec && threadIdx.x == 0) trace_put(p.trace, p.trace_kind + 10u, trace_t0);
 }
 
@@ -334,24 +370,28 @@ void launch_msc_gather(const MscPrepParams& p, int n_streams, cudaStream_t st)
     msc_gather_kernel<<<n_streams * 4, 128, smem, st>>>(p);
 }
 
+template <bool GROUPED> void launch_viterbi_t(const ViterbiParams& p, const int blocks, cudaStream_t st, int stages)
+{
+    cudaFuncSetAttribute(viterbi_kernel<1, GROUPED>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(viterbi_kernel<2, GROUPED>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(viterbi_kernel<3, GROUPED>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+    if (stages == 1) {
+        viterbi_kernel<1, GROUPED><<<blocks, VIT_THREADS, sizeof(VitSmemT<1>), st>>>(p);
+    } else if (stages == 2) {
+        viterbi_kernel<2, GROUPED><<<blocks, VIT_THREADS, sizeof(VitSmemT<2>), st>>>(p);      // 39 KB: fits beside four 46 KB OFDM CTAs on an SM
+    } else {
+        cudaFuncSetAttribute(viterbi_kernel<3, GROUPED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VitSmemT<3>));
+        viterbi_kernel<3, GROUPED><<<blocks, VIT_THREADS, sizeof(VitSmemT<3>), st>>>(p);
+    }
+    if (p.split) viterbi_tb_kernel<GROUPED><<<blocks, VIT_THREADS, 0, st>>>(p);
+}
+
 void launch_viterbi(const ViterbiParams& p_in, cudaStream_t st, int stages)
 {
     ViterbiParams p = p_in; p.one = 1u;
-    const int blocks = (p.n_cw + VIT_THREADS - 1) / VIT_THREADS;
-    cudaFuncSetAttribute(viterbi_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(viterbi_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(viterbi_kernel<3>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    if (stages == 1) {
-        viterbi_kernel<1><<<blocks, VIT_THREADS, sizeof(VitSmemT<1>), st>>>(p);
-    } else if (stages == 2) {
-        viterbi_kernel<2><<<blocks, VIT_THREADS, sizeof(VitSmemT<2>), st>>>(p);      // 39 KB: fits beside four 46 KB OFDM CTAs on an SM
-    } else {
-        cudaFuncSetAttribute(viterbi_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VitSmemT<3>));
-        viterbi_kernel<3><<<blocks, VIT_THREADS, sizeof(VitSmemT<3>), st>>>(p);
-    }
-    if (p.split) viterbi_tb_kernel<<<blocks, VIT_THREADS, 0, st>>>(p);
+    if (p.groups) launch_viterbi_t<true>(p, p.n_groups, st, stages);
+    else launch_viterbi_t<false>(p, (p.n_cw + VIT_THREADS - 1) / VIT_THREADS, st, stages);
 }
-
 
 size_t vit_dec_bytes(int n_cw, int nsteps) { return (size_t)((n_cw + VIT_THREADS - 1) / VIT_THREADS) * nsteps * VIT_THREADS * sizeof(uint2); }
 

@@ -1,6 +1,7 @@
 // viterbi.cuh — parameter blocks and launchers of viterbi.cu / rs.cu
 #pragma once
 #include "common.cuh"
+#include "vit_groups.cuh"
 #include <vector>
 
 namespace dabb {
@@ -32,6 +33,12 @@ struct MscPrepParams {
     int32_t* valid;                   // [n_streams*4] set to 1 for every codeword produced
 };
 
+// one entry of a context's protection-profile table on the device: what a grouped launch (ViterbiParams::groups) takes per CTA
+struct VitProfile {
+    const uint2* steptab; const uint32_t* stage_off; const uint32_t* prbs_words;
+    int32_t nsteps, nbits;
+};
+
 struct ViterbiParams {
     // punctured softbits of codeword cw at frag + (cw / cw_div) * outer_stride + (cw % cw_div) * inner_stride (16-byte aligned, readable
     // up to 160 bytes past the codeword's last softbit); values >= -127
@@ -39,7 +46,10 @@ struct ViterbiParams {
     const uint2* steptab;             // [nsteps] per-step expansion entries (build_vit_tables)
     const uint32_t* stage_off;        // [nstages + 1]
     int n_cw, nsteps, nbits;
-    uint2* dec;                       // [(n_cw+127)/128][nsteps][128]
+    uint2* dec;                       // [(n_cw+127)/128][nsteps][128]; grouped: each CTA at its descriptor's dec_off
+    // optional grouped schedule (vit_groups.cuh): CTA b decodes codewords cw_list[groups[b].first ..] with profiles[groups[b].profile];
+    // steptab, stage_off, nsteps, nbits, prbs_words and n_cw are then unused
+    const VitGroup* groups; const int32_t* cw_list; const VitProfile* profiles; int n_groups;
     uint8_t* out; int64_t out_stride; // packed bytes, multiple of 4
     const uint32_t* prbs_words;       // energy-dispersal sequence packed like the output (or nullptr)
     const int32_t* valid;             // optional per-codeword flag

@@ -220,10 +220,15 @@ class Context:
 
     def select_subchannel(self, start_cu, length_cu, bitrate, eep_profile_a=True, eep_level=3, short_form=False, uep_level=0,
                           dabplus=True, slot=0, first=0, count=None, subch_id=0):
+        """streams [first, first + count) decode this sub-channel in `slot` (dabb_select_subchannel).  The streams of a slot are
+        independent: each may have its own sub-channel, bitrate, protection and DAB/DAB+, and streams not named here decode on
+        unchanged.  At most DABB_MAX_PROFILES (64) distinct protection profiles per context.  process() then needs msc_stride /
+        sf_stride of at least the largest 3 x bitrate / 15 x bitrate among the streams selected in any slot."""
         sc = Subchannel(subch_id, start_cu, length_cu, bitrate, int(short_form), uep_level, int(eep_profile_a), eep_level, int(dabplus))
         self._ck(self.lib.dabb_select_subchannel(self.h, first, self.n_streams if count is None else count, slot, C.byref(sc)))
 
     def remove_subchannel(self, slot=0, first=0, count=None):
+        """streams [first, first + count) stop decoding `slot`; the slot's other streams decode on unchanged"""
         self._ck(self.lib.dabb_remove_subchannel(self.h, first, self.n_streams if count is None else count, slot))
 
     def process(self, iq, stride, buf_start, buf_len, iq_is_host=False, msc_stride=0, sf_stride=0, want=("results", "fibs"), iq_format=0):

@@ -7,8 +7,8 @@
  * service, dump its logical frames) done for all files in lock-step: every iteration hands each stream's next window of samples
  * to one dabb_process() call (host buffers, copied to the device inside the call), then walks the per-stream result records:
  * FIBs (33-byte records: CRC flag + 32 bytes) go to DIR/<name>.fic, the FIGs feed the stream's service database (fig-db.h), the
- * first audio service is selected as soon as its sub-channel is known (streams with the same protection profile share a slot of
- * the library), logical frames go to DIR/<name>.msc, Reed-Solomon statistics to DIR/<name>.rs.  Streams progress independently
+ * first audio service is selected as soon as its sub-channel is known (every stream's in slot 0 of the library, whatever its bitrate
+ * and protection), logical frames go to DIR/<name>.msc, Reed-Solomon statistics to DIR/<name>.rs.  Streams progress independently
  * (per-stream sample position, acquisition state, end of file).  No signal processing happens here.
  *
  * --tii: transmitter identification of every decoded frame, analysed on the device (dabb_options.decode_tii, tap 9); each measurement
@@ -39,8 +39,6 @@ struct Stream {
     int slot = -1; int bitrate = 0; uint32_t sid = 0;
     long frames = 0, fibs_ok = 0, fibs = 0, logical = 0;
 };
-
-struct Profile { dabb_subchannel sc; };
 
 int bytes_per_sample(int fmt) { return fmt == DABB_IQ_CF32 ? 8 : (fmt == DABB_IQ_U8 || fmt == DABB_IQ_S8) ? 2 : 4; }
 
@@ -100,7 +98,6 @@ int main(int argc, char** argv)
     std::vector<int64_t> buf_start((size_t)S);
     std::vector<dabb_frame_result> res((size_t)S);
     std::vector<uint8_t> fibs((size_t)S * 12 * 32), msc((size_t)S * DABB_MAX_SUBCH * 4 * 1152), sf((size_t)S * DABB_MAX_SUBCH * 5760);
-    std::vector<Profile> profiles;                               /* slot k decodes profiles[k] */
     std::vector<dabb_tii_result> tres(tii ? (size_t)S : 0);
 
     int active = S;
@@ -190,14 +187,7 @@ int main(int argc, char** argv)
                     sc.short_form = u.protectionSettings.shortForm; sc.uep_level = u.protectionSettings.uepLevel;
                     sc.eep_profile_a = u.protectionSettings.eepProfile == EEPProtectionProfile::EEP_A; sc.eep_level = (int)u.protectionSettings.eepLevel;
                     sc.dabplus = c.audioType() == AudioServiceComponentType::DABPlus;
-                    /* streams with the same code geometry share a slot */
-                    int k = -1;
-                    for (size_t q = 0; q < profiles.size(); q++) {
-                        const dabb_subchannel& p = profiles[q].sc;
-                        if (p.bitrate == sc.bitrate && p.short_form == sc.short_form && p.uep_level == sc.uep_level && p.eep_profile_a == sc.eep_profile_a && p.eep_level == sc.eep_level && p.dabplus == sc.dabplus) k = (int)q;
-                    }
-                    if (k < 0 && profiles.size() < DABB_MAX_SUBCH) { profiles.push_back(Profile{sc}); k = (int)profiles.size() - 1; }
-                    if (k < 0) { fprintf(stderr, "batch_decode: %s: more than %d different protection profiles in one batch, not decoding its audio\n", z.name.c_str(), DABB_MAX_SUBCH); z.slot = -2; break; }
+                    const int k = 0;
                     if (dabb_select_subchannel(ctx, s, 1, k, &sc) != DABB_OK) { fprintf(stderr, "batch_decode: %s: %s\n", z.name.c_str(), dabb_last_error(ctx)); z.slot = -2; break; }
                     z.slot = k; z.bitrate = sc.bitrate; z.sid = c.SId;
                     break;
