@@ -18,5 +18,3 @@ PY
 unset DABB_LIB
 one default
 for lib in $(ls variant_*.so 2>/dev/null); do export DABB_LIB=$PWD/$lib; one "$lib"; done
-# A/B: with the high-priority time-sync stream
-DABB_PREFIX_LANE=1 one prefixlane

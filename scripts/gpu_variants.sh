@@ -1,7 +1,7 @@
 #!/bin/bash
-# On the GPU box: a short bench (headline config, no CPU / e2e / side measurements) for the default library, for tail-split settings of
-# the default library (environment switches) and for every variant_*.so built by scripts/build_variants.sh, with the stage + pipeline
-# parity tests for each library.  One line per variant: frames/s, ms/step, ofdm_demod_kernel ms and roofline fraction, Viterbi ms.
+# On the GPU box: a short bench (headline config, no CPU / e2e / side measurements) for the default library and for every variant_*.so
+# built by scripts/build_variants.sh, with the stage + pipeline parity tests for each variant.  One line per variant: frames/s, ms/step,
+# ofdm_demod_kernel ms and roofline fraction, Viterbi ms.
 mkdir -p gpurun_out
 one() {   # label
     python bench.py --no-cpu-baseline --no-e2e --no-other-configs --cfo-hz 0 --steps 10 > gpurun_out/bench_var_$1.json 2> gpurun_out/bench_var_$1.err
@@ -19,11 +19,6 @@ PY
 }
 unset DABB_LIB
 one default "-"
-DABB_TAIL_FRAMES=185 one tail185 "-"
-DABB_TAIL_FRAMES=740 one tail740 "-"
-DABB_TAIL_GROUPS=5 one tailg5 "-"
-DABB_TAIL_GROUPS=25 one tailg25 "-"
-DABB_TAIL_FRAMES=740 DABB_TAIL_GROUPS=25 one tail740g25 "-"
 for lib in $(ls variant_*.so 2>/dev/null); do
     export DABB_LIB=$PWD/$lib
     t=$(python -m pytest tests/test_gpu_stages.py tests/test_gpu_pipeline.py -m gpu -q 2>&1 | tail -1)

@@ -87,22 +87,21 @@ struct StepOut {
 
 struct dabb_ctx {
     int device = 0; cudaStream_t stream = nullptr; cudaStream_t streamB = nullptr; cudaEvent_t evA[2] = {nullptr, nullptr}, evB[2] = {nullptr, nullptr}; bool evB_valid[2] = {false, false};
-    int64_t step = 0; int last_parity = 0; DevBuf<int32_t> d_fic_ratio, d_coarse; int ofdm_smem_floor = 0; int vit_stages_now = 3;
-    int prio_b = 0; cudaStream_t streamP = nullptr; cudaEvent_t evPre = nullptr, evPost = nullptr;      // time-sync kernels of lane A at the highest priority (see dabb_create)
+    int64_t step = 0; int last_parity = 0; DevBuf<int32_t> d_fic_ratio, d_coarse;
     cudaStream_t stream2 = nullptr; cudaEvent_t ev_ofdm = nullptr, ev_fic = nullptr; DevBuf<uint2> d_dec_fic; int S = 0; int fft_mode = 0; int disable_coarse = 0; int keep_taps = 0; int placement = 0; int freqsync = 0;
     int decode_tii = 0; DevBuf<float2> d_tii;
     // TII analysis (tii.cu), allocated when decode_tii is first set: the null symbol when keep_taps has no tap for it, each stream's open
     // combinations and their phase-error sums, the step's analyses, the tie-order tables and the step's records (tap 9)
     DevBuf<float2> d_tii_null; DevBuf<dabb_tii::StreamHdr> d_tii_hdr; DevBuf<dabb_tii::Job> d_tii_jobs; DevBuf<int32_t> d_tii_njobs;
     DevBuf<uint32_t> d_tii_sums; DevBuf<uint16_t> d_tii_rank; DevBuf<dabb_tii_result> d_tii_res;
-    bool persistent = false; DevBuf<unsigned int> d_work; TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0;
+    TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0;
     DevBuf<unsigned long long> d_trace_rec; DevBuf<unsigned int> d_trace_count;      // what `trace` points into
     std::string err; int64_t launches = 0; int osc_mismatches = -1; int osc_patched = 0; std::vector<float2> h_osc;
     HostTables* host = nullptr; DevTables dev{};
     DevBuf<float2> d_tw_fwd, d_tw_inv, d_prs_ref, d_osc; DevBuf<int16_t> d_invperm, d_fic_map; DevBuf<uint8_t> d_gf_exp, d_gf_log, d_prbs; DevBuf<double2> d_osc_hi;   // what `dev` points into
     DevBuf<StreamState> d_state; DevBuf<StepScratch> d_scr; DevBuf<MscSlotState> d_slots;
     DevBuf<int64_t> d_buf_start, d_win, d_prs; DevBuf<int32_t> d_nco_sync, d_nco_frame;
-    DevBuf<int32_t> d_active, d_index; DevBuf<float> d_cir, d_cir_work; int search_generic = 0; int vit_split = 0; DevBuf<float2> d_r1, d_null; DevBuf<int32_t> d_snr; DevBuf<float2> d_fc; DevBuf<float> d_lvl;
+    DevBuf<int32_t> d_active, d_index; DevBuf<float> d_cir, d_cir_work; int search_generic = 0; DevBuf<float2> d_r1, d_null; DevBuf<int32_t> d_snr; DevBuf<float2> d_fc; DevBuf<float> d_lvl;
     DevBuf<int8_t> d_soft; DevBuf<uint2> d_fic_steptab; DevBuf<uint32_t> d_fic_stage_off; DevBuf<uint2> d_dec; DevBuf<uint8_t> d_fibs; DevBuf<int32_t> d_crc;
     DevBuf<dabb_frame_result> d_results;
     // the protection-profile table: one entry per distinct ProtProfile a select call has met, built the first time it is selected and
@@ -138,7 +137,7 @@ struct dabb_ctx {
         std::vector<int32_t> flen;      // [slot][stream] the stream's logical frame length when the step was enqueued (0: nothing to deliver)
     } pend[2], pend_sync;     // the two dabb_submit slots; dabb_process and taps 7 / 8, which never leave a step outstanding
     int pend_head = 0, pend_count = 0; int64_t submits = 0;
-    int groups = 1; int fc_pitch = 1; int tail_frames = 0; int tail_groups = 5; int nco_fast = 0;
+    int groups = 1; int fc_pitch = 1; int tail_frames = 0; int nco_fast = 0;
     DevBuf<const int32_t*> d_info_tab;
     // optional per-kernel timing: one event after every launch, durations = differences of consecutive events
     bool prof = false; std::vector<cudaEvent_t> prof_ev; std::vector<const char*> prof_name; size_t prof_used = 0;
@@ -449,7 +448,6 @@ __global__ void set_slot_kernel(MscSlotState* slots, int n_slots, int slot, int 
 void sync_all(dabb_ctx* ctx)
 {
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    if (ctx->streamP) cudaStreamSynchronize(ctx->streamP);
     if (ctx->streamB) cudaStreamSynchronize(ctx->streamB);
     if (ctx->stream2) cudaStreamSynchronize(ctx->stream2);
     if (ctx->streamC) cudaStreamSynchronize(ctx->streamC);
@@ -667,41 +665,15 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     ctx->nco_fast = cfg->nco_mode == DABB_NCO_FAST;
     auto fail = [&](int code) { g_create_error = ctx->err; dabb_destroy(ctx); return code; };
     if (cudaSetDevice(ctx->device) != cudaSuccess) { ctx->err = "cudaSetDevice failed"; return fail(DABB_E_CUDA); }
-    // Stream priorities.  Lane A (time sync + OFDM of frame n+1) and lane B (FIC / MSC Viterbi + RS of frame n) become runnable at the
-    // same moment; lane B gets the higher priority and runs first, in a burst (its CTAs take every slot the OFDM launch frees).
-    // DABB_LANES=partition is the measured alternative (DESIGN.md 3.3, CTA timelines with DABB_TRACE): lane A higher, the OFDM kernel
-    // persistent and capped at four CTAs per SM by a 45 KB shared-memory request, so that one two-buffer Viterbi CTA (16 384 registers,
-    // 40 KB) runs beside them for the whole launch.  The two kernels then do share every SM - and slow each other down by as much as
-    // they overlap (OFDM 3.2 -> 4.3 ms with the Viterbi CTAs beside it; step 4.94 vs 4.70 ms), so the burst order stays the default.
-    const char* lanes_env = getenv("DABB_LANES");
-    const bool partition = lanes_env ? !strcmp(lanes_env, "partition") : false;
+    // Two lanes (enqueue_step): lane A (ctx->stream: time sync + OFDM of frame n+1) and lane B (streamB: MSC + RS of frame n, with its
+    // FIC chain on stream2, which overlaps the MSC chain; both only depend on the OFDM kernel) become runnable at the same moment.  Lane B
+    // gets the higher priority and runs first, in a burst: its CTAs take every slot the OFDM launch frees.  (Sharing the SMs instead, with
+    // the OFDM kernel capped so that a Viterbi CTA fits beside it, slowed the OFDM kernel by as much as the two overlapped; DESIGN.md 3.3.)
     int prio_lo = 0, prio_hi = 0; cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-    if (cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, partition ? prio_hi : prio_lo) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return fail(DABB_E_CUDA); }
-    // lane B (FIC/MSC/RS of frame n) runs on its own stream so that it overlaps lane A (time sync + OFDM of frame n+1)
-    {
-        int lo = 0, hi = 0; cudaDeviceGetStreamPriorityRange(&lo, &hi);   // lane B gets the higher priority: its CTAs take the SM resources lane A leaves free
-        // Three levels where the device has them: the short time-sync kernels that precede the OFDM kernel (plan, findIndex, post_sync:
-        // 0.2 ms) > lane B > the OFDM kernel.  With only two levels the block scheduler serves lane B's grids first and the time sync of
-        // frame n+1 crawls in the slots the Viterbi CTAs leave - the CTA timelines showed 0.6 ms per step with Viterbi CTAs alone on the
-        // GPU because the OFDM launch behind that time sync had not started (DESIGN.md 3.3).  Measured: no gain (the Viterbi kernel runs at
-        // full speed in that phase, and beside OFDM CTAs it does not), so it is an experiment switch: DABB_PREFIX_LANE=1.
-        const bool prefix = !partition && getenv("DABB_PREFIX_LANE") && atoi(getenv("DABB_PREFIX_LANE")) == 1 && hi < lo - 1;
-        const int prio_b = prefix ? hi + 1 : hi;
-        if (prefix) {
-            if (cudaStreamCreateWithPriority(&ctx->streamP, cudaStreamNonBlocking, hi) != cudaSuccess ||
-                cudaEventCreateWithFlags(&ctx->evPre, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&ctx->evPost, cudaEventDisableTiming) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return fail(DABB_E_CUDA); }
-        }
-        ctx->prio_b = prio_b;
-        if (cudaStreamCreateWithPriority(&ctx->streamB, cudaStreamNonBlocking, partition ? lo : prio_b) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return fail(DABB_E_CUDA); }
-        // co-residency experiment: 46 KB per OFDM CTA -> four of them per SM (49 152 registers, 188 KB), leaving exactly the 16 384 registers
-        // and 40 KB one two-stage Viterbi CTA needs, so that the integer ACS work runs in the issue slots the shared-memory-bound OFDM
-        // kernel leaves free instead of taking turns with it
-        ctx->ofdm_smem_floor = (getenv("DABB_CORESIDENT") || partition) ? 45 * 1024 : 0;
-        ctx->persistent = partition;
-    }
+    if (cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, prio_lo) != cudaSuccess ||
+        cudaStreamCreateWithPriority(&ctx->streamB, cudaStreamNonBlocking, prio_hi) != cudaSuccess ||
+        cudaStreamCreateWithPriority(&ctx->stream2, cudaStreamNonBlocking, prio_hi) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return fail(DABB_E_CUDA); }
     for (int i = 0; i < 2; i++) if (cudaEventCreateWithFlags(&ctx->evA[i], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&ctx->evB[i], cudaEventDisableTiming) != cudaSuccess) { ctx->err = "event creation failed"; return fail(DABB_E_CUDA); }
-    // second stream: the FIC chain (de-puncture, Viterbi, CRC) overlaps the MSC chain; both only depend on the OFDM kernel
-    { int lo = 0, hi = 0; cudaDeviceGetStreamPriorityRange(&lo, &hi); if (cudaStreamCreateWithPriority(&ctx->stream2, cudaStreamNonBlocking, partition ? lo : ctx->prio_b) != cudaSuccess) { ctx->err = "cudaStreamCreate failed"; return fail(DABB_E_CUDA); } }
     if ( cudaEventCreateWithFlags(&ctx->ev_ofdm, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&ctx->ev_fic, cudaEventDisableTiming) != cudaSuccess) { ctx->err = "stream/event creation failed"; return fail(DABB_E_CUDA); }
     ctx->host = new HostTables();
@@ -709,10 +681,7 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     const int S = ctx->S;
     int rc = 0;
     ctx->tail_frames = (cfg->ofdm_tail_split == 0 && ctx->groups == 1) ? ofdm_tail_frames(S) : 0;
-    if (ctx->tail_frames && getenv("DABB_TAIL_FRAMES")) { const int v = atoi(getenv("DABB_TAIL_FRAMES")); if (v >= 0 && v <= S) ctx->tail_frames = v; }   // experiments
-    ctx->tail_groups = 5;            // 16-symbol CTAs: measured best of 5 / 15 / 25 (3.207 -> 3.199 ms per 8192 frames)
-    if (getenv("DABB_TAIL_GROUPS")) { const int v = atoi(getenv("DABB_TAIL_GROUPS")); if (v > 0 && 75 % v == 0) ctx->tail_groups = v; }
-    ctx->fc_pitch = ctx->tail_frames ? ctx->tail_groups : ctx->groups;
+    ctx->fc_pitch = ctx->tail_frames ? OFDM_TAIL_GROUPS : ctx->groups;
     // tables
     auto& tf = ctx->d_tw_fwd; auto& ti = ctx->d_tw_inv; auto& pr = ctx->d_prs_ref; auto& osc = ctx->d_osc; auto& ip = ctx->d_invperm; auto& fm = ctx->d_fic_map;
     auto& ge = ctx->d_gf_exp; auto& gl = ctx->d_gf_log; auto& pb = ctx->d_prbs;
@@ -737,7 +706,7 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     ctx->dev.gf_exp = ge; ctx->dev.gf_log = gl; ctx->dev.prbs = pb;
     {
         // on-the-fly oscillator: upload the factors, compare against the table for every index on the device, adopt it only when
-        // nothing differs; DABB_OSC_TABLE=1 in the environment forces the table lookups (A/B measurements)
+        // nothing differs (else the kernels keep the table lookups)
         auto& hi = ctx->d_osc_hi;
         if ((rc = dalloc(ctx, hi, 2000))) return fail(rc);
         std::vector<double2> h_hi(2000);
@@ -746,7 +715,7 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
         cudaStreamSynchronize(ctx->stream);
         ctx->dev.osc_hi = hi; ctx->dev.osc_mode = 0;
         ctx->osc_mismatches = launch_osc_verify(ctx->dev, ctx->stream);
-        if (ctx->osc_mismatches == 0 && !getenv("DABB_OSC_TABLE")) ctx->dev.osc_mode = 1;
+        if (ctx->osc_mismatches == 0) ctx->dev.osc_mode = 1;
         std::vector<float2>().swap(ctx->h_osc);
     }
     {
@@ -760,7 +729,6 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
         cudaMemcpy(ctx->d_fic_steptab, steps.data(), steps.size() * sizeof(uint2), cudaMemcpyHostToDevice);
         cudaMemcpy(ctx->d_fic_stage_off, soff.data(), soff.size() * 4, cudaMemcpyHostToDevice);
     }
-    ctx->vit_split = getenv("DABB_VIT_SPLIT") ? atoi(getenv("DABB_VIT_SPLIT")) : 0;       // traceback as its own launch (A/B)
     ctx->search_generic = getenv("DABB_SEARCH_GENERIC") != nullptr;     // A/B: ThresholdBeforePeak through the literal sliding maximum
     if (getenv("DABB_TRACE")) {
         ctx->trace_path = getenv("DABB_TRACE"); ctx->trace.cap = 1u << 20;
@@ -815,9 +783,6 @@ void dabb_destroy(dabb_ctx* ctx)
     if (ctx->ev_ofdm) cudaEventDestroy(ctx->ev_ofdm);
     if (ctx->ev_fic) cudaEventDestroy(ctx->ev_fic);
     for (int i = 0; i < 2; i++) { if (ctx->evA[i]) cudaEventDestroy(ctx->evA[i]); if (ctx->evB[i]) cudaEventDestroy(ctx->evB[i]); }
-    if (ctx->streamP) cudaStreamDestroy(ctx->streamP);
-    if (ctx->evPre) cudaEventDestroy(ctx->evPre);
-    if (ctx->evPost) cudaEventDestroy(ctx->evPost);
     if (ctx->streamB) cudaStreamDestroy(ctx->streamB);
     if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -910,8 +875,8 @@ static int run_fic(dabb_ctx* ctx, const int8_t* soft, int64_t soft_stride, const
     vp.frag = soft; vp.cw_div = 4; vp.outer_stride = soft_stride; vp.inner_stride = 2304; vp.steptab = ctx->d_fic_steptab; vp.stage_off = ctx->d_fic_stage_off;
     vp.n_cw = n_frames * 4; vp.nsteps = 774; vp.nbits = 768;
     vp.dec = dec; vp.out = fibs; vp.out_stride = 96; vp.prbs_words = ctx->d_fic_prbs_words; vp.valid = nullptr;
-    vp.trace = ctx->trace; vp.trace_kind = 2; vp.split = ctx->vit_split;
-    launch_viterbi(vp, st, ctx->vit_stages_now);
+    vp.trace = ctx->trace; vp.trace_kind = 2;
+    launch_viterbi(vp, st);
     if ((rc = check_launch(ctx, "viterbi_kernel(FIC)"))) return rc;
     launch_fic_crc(fibs, active, n_frames, crc, st);
     return check_launch(ctx, "fic_crc_kernel");
@@ -972,8 +937,6 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     // serially on the main stream.
     const int par = (int)(ctx->step & 1);
     const bool serial = ctx->prof;
-    // three staging buffers by default; DABB_LANES=partition uses two (39 KB) so that one Viterbi CTA fits beside four OFDM CTAs
-    ctx->vit_stages_now = getenv("DABB_VIT_STAGES") ? atoi(getenv("DABB_VIT_STAGES")) : (ctx->persistent && !serial ? 2 : 3);
     cudaStream_t A = ctx->stream, B = serial ? ctx->stream : ctx->streamB;
     StepScratch* scr = ctx->d_scr + (size_t)par * S;
     int64_t* d_win = ctx->d_win + (size_t)par * S; int64_t* d_prs = ctx->d_prs + (size_t)par * S;
@@ -984,10 +947,6 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
 
     // the buffers of this parity were last used by lane B two frames ago
     if (!serial && ctx->evB_valid[par]) CK(cudaStreamWaitEvent(A, ctx->evB[par], 0));
-    // the time-sync kernels run on the highest-priority stream: it inherits everything lane A has waited for so far (previous step, input
-    // copies, buffer hand-back) through one event, and lane A continues behind its last kernel
-    cudaStream_t A_low = A;
-    if (!serial && ctx->streamP) { CK(cudaEventRecord(ctx->evPre, A)); CK(cudaStreamWaitEvent(ctx->streamP, ctx->evPre, 0)); A = ctx->streamP; }
     CK(cudaMemcpyAsync(ctx->d_buf_start, io->buf_start, sizeof(int64_t) * S, cudaMemcpyHostToDevice, A));
     prof_mark(ctx, "__step_begin");
     const int tb = 128, gb = (S + tb - 1) / tb;
@@ -1009,18 +968,10 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     }
     post_sync_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, d_index, ctx->disable_coarse ? nullptr : ctx->d_coarse.get(), S, d_prs, d_nco_frame, d_active);
     if ((rc = check_launch(ctx, "post_sync_kernel"))) return rc;
-    if (A != A_low) { CK(cudaEventRecord(ctx->evPost, A)); A = A_low; CK(cudaStreamWaitEvent(A, ctx->evPost, 0)); }
     OfdmParams op{}; op.iq = iq; op.stride = stride; op.prs_start = d_prs; op.nco = d_nco_frame; op.active = d_active; op.soft = d_soft; op.soft_stride = DABB_SOFT_PER_FRAME;
     op.r1 = ctx->d_r1; op.freqcorr = d_fc; op.level = d_lvl; op.snr = d_snr; op.n_frames = S; op.groups = ctx->groups; op.sym_per_cta = 75 / ctx->groups;
     op.trace = ctx->trace;
-    if (ctx->persistent && !serial) {
-        if (!ctx->d_work && (rc = dalloc(ctx, ctx->d_work, 1))) return rc;
-        CK(cudaMemsetAsync(ctx->d_work, 0, sizeof(unsigned int), A));
-        op.work = ctx->d_work;
-    }
-    op.n_full = S - ctx->tail_frames; op.tail_groups = ctx->tail_frames ? ctx->tail_groups : 1; op.fc_pitch = ctx->fc_pitch; op.nco_fast = ctx->nco_fast;
-    // pipelined mode: 50 KB per CTA -> four OFDM CTAs per SM, leaving registers and 23 KB of shared memory for one lane-B CTA
-    op.smem_floor = (serial && !getenv("DABB_CORESIDENT_SERIAL")) ? 0 : ctx->ofdm_smem_floor;     // DABB_CORESIDENT_SERIAL: time the capped kernel alone
+    op.n_full = S - ctx->tail_frames; op.tail_groups = ctx->tail_frames ? OFDM_TAIL_GROUPS : 1; op.fc_pitch = ctx->fc_pitch; op.nco_fast = ctx->nco_fast;
     launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, A);
     if ((rc = check_launch(ctx, "ofdm_demod_kernel"))) return rc;
     advance_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, S, ctx->fc_pitch, d_fc, d_lvl);
@@ -1067,8 +1018,8 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         ViterbiParams vp{}; vp.frag = sl.d_frag; vp.cw_div = 1; vp.outer_stride = sl.frag_pitch; vp.inner_stride = 0;
         vp.groups = sl.d_groups; vp.cw_list = sl.d_cw_list; vp.profiles = ctx->d_profiles; vp.n_groups = sl.n_groups;
         vp.n_cw = S * 4; vp.dec = sl.d_dec; vp.out = sl.d_logical; vp.out_stride = sl.flen_pad; vp.valid = sl.d_valid;
-        vp.trace = ctx->trace; vp.trace_kind = 3; vp.split = ctx->vit_split;
-        launch_viterbi(vp, B, ctx->vit_stages_now);
+        vp.trace = ctx->trace; vp.trace_kind = 3;
+        launch_viterbi(vp, B);
         if ((rc = check_launch(ctx, "viterbi_kernel(MSC)"))) return rc;
         SuperframeParams fp{}; fp.active = d_active; fp.slots = ctx->d_slots; fp.n_slots = ctx->n_slots; fp.slot = k; fp.n_streams = S; fp.logical = sl.d_logical; fp.logical_stride = sl.flen_pad;
         fp.valid = sl.d_valid; fp.window = sl.d_window; fp.window_pitch = 5 * sl.flen_pad; fp.sf_out = sl.d_sf; fp.sf_pitch = 5 * sl.flen_pad; fp.info = sl.d_info; fp.gf_exp = ctx->dev.gf_exp; fp.gf_log = ctx->dev.gf_log;

@@ -57,8 +57,6 @@ struct OfdmParams {
     int fc_pitch;                                // freqcorr entries per frame (>= groups, tail_groups); 0 -> the larger of the two
     int nco_fast;                                // DABB_NCO_FAST: fp32 oscillator (tolerance mode)
     TraceBuf trace;                              // rec == nullptr: off
-    unsigned int* work;                          // persistent launch: item counter (zeroed by the caller before the launch); nullptr: one CTA per item
-    int smem_floor;                              // request at least this much dynamic shared memory (caps CTAs/SM so that other kernels fit beside it)
 };
 
 struct SyncParams {
@@ -78,6 +76,7 @@ struct SyncParams {
 
 void launch_ofdm_demod(const DevTables& tb, const OfdmParams& p, int fft_mode, cudaStream_t st);
 int ofdm_tail_frames(int n_frames);
+constexpr int OFDM_TAIL_GROUPS = 5;              // CTAs per tail frame (15 data symbols each): the best of 5 / 15 / 25 before the port to H100
 void launch_find_index(const DevTables& tb, const SyncParams& p, int fft_mode, cudaStream_t st, int part = -1);
 void launch_tii_spectra(const DevTables& tb, const float2* iq, int64_t stride, const int64_t* prs_start, const int32_t* nco_frame, const int32_t* active,
                         const float2* nulls, float2* out, int n, cudaStream_t st);

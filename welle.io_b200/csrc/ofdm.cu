@@ -199,7 +199,6 @@ struct __align__(16) DemodSmem {
     float2 tw[TwLayout::C4];         // 1 KB: twiddles of passes A and B (pass C reads its 15 KB through L1 with __ldg)
     uint16_t sbuf[1536 + 128];        // (re | im << 8) per logical carrier: one 16-bit scatter store per carrier
 #endif
-    int item;                        // persistent launch: the work item all threads of the CTA process next
     float2 rtab[2][16];              // DABB_NCO_FAST: e^{-j theta((128 h + 256 c) Hz)} for the PRS / the data symbols
     float red[16];
     uint64_t full;
@@ -347,23 +346,13 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
     const int rslot = t < 96 ? (((int)tb.invperm[2 * TU + t] & 0xFF) | (((int)tb.invperm[2 * TU + t + 96] & 0xFF) << 8) |
                                (((int)tb.invperm[2 * TU + t] >> 8) << 16) | (((int)tb.invperm[2 * TU + t + 96] >> 8) << 17)) : 0;
     uint32_t parity = 0;
-    const int n_items = p.n_full * p.groups + (p.n_frames - p.n_full) * p.tail_groups;
     __syncthreads();
 
-    // Work items: the first n_full frames are walked by `groups` items each; the remaining (tail) frames are cut into tail_groups short
-    // items, which come last and fill the slots the long ones free one by one at the end of the launch.  Classic launch (p.work ==
-    // nullptr): one CTA per item.  Persistent launch: a fixed set of CTAs (as many as are resident at once) pulls items from a counter -
-    // a grid with no undispatched CTAs, so that the block scheduler hands the SM resources this kernel cannot use (the slot its
-    // shared-memory request leaves free) to the other lane's kernels while it runs (DESIGN.md 3.3).
-    for (int item = p.work ? -1 : (int)blockIdx.x; ; ) {
-        if (p.work) {
-            __syncthreads();                                  // the previous item is finished by every thread (inbuf, xbuf, red reusable)
-            if (t == 0) sm.item = (int)atomicAdd(p.work, 1u);
-            __syncthreads();
-            item = sm.item;
-        }
-        if (item >= n_items) break;
-        [&]() {
+    // One CTA per work item: the first n_full frames are walked by `groups` items each; the remaining (tail) frames are cut into
+    // tail_groups short items, which come last and fill the slots the long ones free one by one at the end of the launch.
+    const int item = blockIdx.x;
+    if (item >= p.n_full * p.groups + (p.n_frames - p.n_full) * p.tail_groups) return;
+    [&]() {     // the body stays a lambda: as a plain block, ptxas spills more in three of the eight instances
     int f, g, spc, ng;
     if (item < p.n_full * p.groups) { f = item / p.groups; g = item % p.groups; spc = p.sym_per_cta; ng = p.groups; }
     else { const int r = item - p.n_full * p.groups; f = p.n_full + r / p.tail_groups; g = r % p.tail_groups; spc = 75 / p.tail_groups; ng = p.tail_groups; }
@@ -491,9 +480,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
         if (g == 0 && t > 0 && t < p.fc_pitch - ng + 1) p.level[(int64_t)f * p.fc_pitch + ng - 1 + t] = 0.f;
     }
     if (p.trace.rec && t == 0) trace_put(p.trace, 1u, trace_t0);
-        }();
-        if (!p.work) break;
-    }
+    }();
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -980,18 +967,8 @@ void launch_ofdm_demod(const DevTables& tb, const OfdmParams& p_in, int fft_mode
     if (p.tail_groups < 1 || 75 % p.tail_groups) { p.tail_groups = 1; }
     if (p.n_full < 0 || p.n_full > p.n_frames || p.tail_groups == 1) p.n_full = p.n_frames;
     if (p.fc_pitch < 1) p.fc_pitch = p.groups > p.tail_groups ? p.groups : p.tail_groups;
-    const size_t sm = sizeof(DemodSmem) > (size_t)p.smem_floor ? sizeof(DemodSmem) : (size_t)p.smem_floor;
-    int n_ctas = p.n_full * p.groups + (p.n_frames - p.n_full) * p.tail_groups;
-    if (p.work) {
-        // persistent: as many CTAs as are resident at once with this shared-memory request
-        int dev = 0, sms = 0, per_sm = 0;
-        cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        set_smem(ofdm_demod_kernel<true, false, false>, sm);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ofdm_demod_kernel<true, false, false>, OFDM_THREADS, sm);
-        const int resident = sms * (per_sm > 0 ? per_sm : 1);
-        if (n_ctas > resident) n_ctas = resident;
-    }
-    const dim3 grid(n_ctas), block(OFDM_THREADS);
+    const size_t sm = sizeof(DemodSmem);
+    const dim3 grid(p.n_full * p.groups + (p.n_frames - p.n_full) * p.tail_groups), block(OFDM_THREADS);
     const bool tap = p.r1 != nullptr, fast = p.nco_fast != 0 && p.nco != nullptr;
 #define LAUNCH(E, T, F) do { set_smem(ofdm_demod_kernel<E, T, F>, sm); ofdm_demod_kernel<E, T, F><<<grid, block, sm, st>>>(tb, p); } while (0)
 #define LAUNCH_F(E, T) do { if (fast) LAUNCH(E, T, true); else LAUNCH(E, T, false); } while (0)

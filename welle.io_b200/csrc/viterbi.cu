@@ -127,10 +127,11 @@ constexpr int VIT_THREADS = VIT_THREADS_N;     // codewords per CTA
 constexpr int VIT_MIN_CTAS = 512 / VIT_THREADS;   // 512 threads of 128 registers per SM
 constexpr int VIT_ROW_PITCH = 144;      // 128 B of softbits + 16 B pad (rows stay 16-byte aligned for the bulk copies)
 constexpr int VIT_STAGE_BYTES = VIT_THREADS * VIT_ROW_PITCH;
+constexpr int VIT_STAGES = 3;           // depth of the staging ring: stage s + 3 is requested while stage s is decoded
 
 constexpr int VIT_WARPS = VIT_THREADS / 32;
 constexpr int VIT_TAB_BYTES = VIT_STAGE_STEPS * 8;      // one stage's expansion entries (24 x 8 bytes = 12 x 16)
-template <int VIT_STAGES> struct __align__(16) VitSmemT {
+struct __align__(16) VitSmem {
     unsigned char stage[VIT_STAGES][VIT_STAGE_BYTES];        // per thread: the 128 bytes that hold its next <= 96 softbits
     unsigned char tab[VIT_STAGES][VIT_WARPS][VIT_TAB_BYTES]; // per warp: the stage's expansion entries
 };
@@ -210,12 +211,11 @@ __device__ __forceinline__ void viterbi_traceback(const ViterbiParams& p, const 
 // addresses from uniform registers, so the compiler emitted a 32-iteration lane loop per warp and stage - ncu: 10 % of the samples.)
 // The stage's expansion entries (the same for all codewords) are copied once per WARP by twelve of its lanes into a warp-private
 // area and read after a __syncwarp: no __syncthreads in the loop at all.
-// VIT_STAGES = 3: stand-alone launches (deep prefetch).  VIT_STAGES = 1: 19 KB of shared memory (co-residency experiment).
-template <int VIT_STAGES, bool GROUPED>
+template <bool GROUPED>
 __device__ __forceinline__ void viterbi_cta(const ViterbiParams& p, const int block)
 {
     extern __shared__ __align__(16) unsigned char smraw[];
-    VitSmemT<VIT_STAGES>& sm = *reinterpret_cast<VitSmemT<VIT_STAGES>*>(smraw);
+    VitSmem& sm = *reinterpret_cast<VitSmem*>(smraw);
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     const unsigned long long trace_t0 = p.trace.rec ? trace_now() : 0ull;
     VitJob job;
@@ -288,30 +288,15 @@ __device__ __forceinline__ void viterbi_cta(const ViterbiParams& p, const int bl
     }
     cp_async_wait<0>();
     if (p.trace.rec && t == 0) trace_put(p.trace, p.trace_kind, trace_t0);       // forward pass of thread 0 done
-    if (p.split) return;                 // the traceback runs as its own launch (viterbi_tb_kernel)
     if (!have) return;
     viterbi_traceback(p, cw, dec, vit_job_nbits<GROUPED>(p, job), vit_job_prbs<GROUPED>(p, job));
     if (p.trace.rec && t == 0) trace_put(p.trace, p.trace_kind + 10u, trace_t0);  // ... and its traceback
 }
 
 // GROUPED: the MSC launch of a sub-channel slot (ViterbiParams::groups); the FIC and the stage-level entry points use the plain form
-template <int VIT_STAGES, bool GROUPED>
-__global__ void __launch_bounds__(VIT_THREADS, VIT_MIN_CTAS)
-viterbi_kernel(ViterbiParams p) { viterbi_cta<VIT_STAGES, GROUPED>(p, blockIdx.x); }
-
-// the traceback as its own launch (ViterbiParams::split, DABB_VIT_SPLIT=1): a serial walk per codeword bound by the latency of its
-// decision loads, without shared memory, so that the SMs can take the next kernels' CTAs beside it - which the fused kernel's 57 KB
-// CTAs keep out while they walk.  Measured: no gain (4.45 vs 4.43 ms per step), so the fused form stays the default.
 template <bool GROUPED>
-__global__ void __launch_bounds__(VIT_THREADS, 4)
-viterbi_tb_kernel(ViterbiParams p)
-{
-    const unsigned long long trace_t0 = p.trace.rec ? trace_now() : 0ull;
-    VitJob job;
-    if (!viterbi_job<GROUPED>(p, blockIdx.x, threadIdx.x, job) || !job.have) return;
-    viterbi_traceback(p, job.cw, job.dec, vit_job_nbits<GROUPED>(p, job), vit_job_prbs<GROUPED>(p, job));
-    if (p.trace.rec && threadIdx.x == 0) trace_put(p.trace, p.trace_kind + 10u, trace_t0);
-}
+__global__ void __launch_bounds__(VIT_THREADS, VIT_MIN_CTAS)
+viterbi_kernel(ViterbiParams p) { viterbi_cta<GROUPED>(p, blockIdx.x); }
 
 
 // CRC of the 12 FIBs of a frame (x^16 + x^12 + x^5 + 1, preset ones, inverted remainder; MathHelper.h:53-80): one thread per FIB, 16
@@ -370,27 +355,18 @@ void launch_msc_gather(const MscPrepParams& p, int n_streams, cudaStream_t st)
     msc_gather_kernel<<<n_streams * 4, 128, smem, st>>>(p);
 }
 
-template <bool GROUPED> void launch_viterbi_t(const ViterbiParams& p, const int blocks, cudaStream_t st, int stages)
+template <bool GROUPED> void launch_viterbi_t(const ViterbiParams& p, const int blocks, cudaStream_t st)
 {
-    cudaFuncSetAttribute(viterbi_kernel<1, GROUPED>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(viterbi_kernel<2, GROUPED>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(viterbi_kernel<3, GROUPED>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    if (stages == 1) {
-        viterbi_kernel<1, GROUPED><<<blocks, VIT_THREADS, sizeof(VitSmemT<1>), st>>>(p);
-    } else if (stages == 2) {
-        viterbi_kernel<2, GROUPED><<<blocks, VIT_THREADS, sizeof(VitSmemT<2>), st>>>(p);      // 39 KB: fits beside four 46 KB OFDM CTAs on an SM
-    } else {
-        cudaFuncSetAttribute(viterbi_kernel<3, GROUPED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VitSmemT<3>));
-        viterbi_kernel<3, GROUPED><<<blocks, VIT_THREADS, sizeof(VitSmemT<3>), st>>>(p);
-    }
-    if (p.split) viterbi_tb_kernel<GROUPED><<<blocks, VIT_THREADS, 0, st>>>(p);
+    cudaFuncSetAttribute(viterbi_kernel<GROUPED>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+    cudaFuncSetAttribute(viterbi_kernel<GROUPED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VitSmem));
+    viterbi_kernel<GROUPED><<<blocks, VIT_THREADS, sizeof(VitSmem), st>>>(p);
 }
 
-void launch_viterbi(const ViterbiParams& p_in, cudaStream_t st, int stages)
+void launch_viterbi(const ViterbiParams& p_in, cudaStream_t st)
 {
     ViterbiParams p = p_in; p.one = 1u;
-    if (p.groups) launch_viterbi_t<true>(p, p.n_groups, st, stages);
-    else launch_viterbi_t<false>(p, (p.n_cw + VIT_THREADS - 1) / VIT_THREADS, st, stages);
+    if (p.groups) launch_viterbi_t<true>(p, p.n_groups, st);
+    else launch_viterbi_t<false>(p, (p.n_cw + VIT_THREADS - 1) / VIT_THREADS, st);
 }
 
 size_t vit_dec_bytes(int n_cw, int nsteps) { return (size_t)((n_cw + VIT_THREADS - 1) / VIT_THREADS) * nsteps * VIT_THREADS * sizeof(uint2); }

@@ -55,7 +55,6 @@ struct ViterbiParams {
     const int32_t* valid;             // optional per-codeword flag
     TraceBuf trace; uint32_t trace_kind;    // optional CTA timeline (common.cuh)
     uint32_t one;                     // = 1 (set by the launcher; keeps a multiply-add opaque to the assembler, see viterbi_core.cuh)
-    int split;                        // 1: forward pass and traceback as two launches (viterbi_kernel, then viterbi_tb_kernel)
 };
 
 
@@ -65,7 +64,7 @@ void build_vit_tables_u2(const int16_t* map, int nsteps, std::vector<uint2>& ste
 void launch_clamp_copy(const int8_t* src, int8_t* dst, int64_t n, cudaStream_t st);
 void launch_msc_collect(const MscCollectParams& p, int n_streams, cudaStream_t st);
 void launch_msc_gather(const MscPrepParams& p, int n_streams, cudaStream_t st);
-void launch_viterbi(const ViterbiParams& p, cudaStream_t st, int stages = 3);
+void launch_viterbi(const ViterbiParams& p, cudaStream_t st);
 void launch_fic_crc(const uint8_t* fibs, const int32_t* active, int n_frames, int32_t* mask_out, cudaStream_t st);
 void launch_unpack_bits(const uint8_t* bytes, int64_t stride, int n_cw, int nbits, uint8_t* bits, cudaStream_t st);
 
