@@ -65,7 +65,7 @@ typedef struct {
     int32_t disable_coarse;     /* RadioReceiverOptions::disableCoarseCorrector (radio-receiver-options.h:66-85) */
     int32_t keep_taps;          /* 1: keep CIR / softbits / constellation / null symbol of the last frame readable via dabb_read_tap */
     int32_t n_subch_slots;      /* sub-channels decodable per stream at once (1..DABB_MAX_SUBCH), 0 -> 1 */
-    int32_t max_subch_cu;       /* largest selectable sub-channel in capacity units, 0 -> 144 */
+    int32_t max_subch_cu;       /* largest selectable sub-channel in capacity units, 0 -> 144; values above 864 (the whole MSC) are taken as 864 */
     int32_t ofdm_groups;        /* CTAs per frame in the OFDM kernel (divisor of 75), 0 -> chosen from n_streams */
     int32_t fft_placement;      /* DABB_PLACEMENT_* (PhaseReference::findIndex variant) */
     int32_t freqsync_method;    /* DABB_FREQSYNC_* (OFDMProcessor::processPRS variant) */

@@ -215,7 +215,7 @@ class Oracle:
         cfg.dabplus = int(dabplus); cfg.select_after_frames = select_after_frames
         rx = C.c_void_p(self.lib.orc_rx_new(C.byref(cfg)))
         nfr = len(iq) // TF + 2
-        fibs = np.zeros(33 * 12 * nfr, np.uint8); msc = np.zeros(4 * nfr * 3 * 384, np.uint8)
+        fibs = np.zeros(33 * 12 * nfr, np.uint8); msc = np.zeros(4 * nfr * 3 * (prot.bitrate if prot is not None else 0), np.uint8)
         rs = np.zeros(2 * 4 * nfr, np.int32); fi = (FrameInfo * nfr)()
         soft = np.zeros(want_soft * 75 * 3072, np.int8) if want_soft else None
         nf_, nm_, nr_ = C.c_long(), C.c_long(), C.c_long()

@@ -948,6 +948,7 @@ long orc_rx_run(orc_rx_t* r, const float* iq, long nsamples,
     int8_t* dtmp = frag ? (int8_t*)malloc(frag) : NULL;
     uint8_t* obits = frag ? (uint8_t*)malloc(24 * r->cfg.prot.bitrate) : NULL;
     const int flen = 3 * r->cfg.prot.bitrate;
+    uint8_t* fr = frag ? (uint8_t*)malloc(flen) : NULL;
 
     if (!r->started) {
         r->started = 1;
@@ -1025,7 +1026,6 @@ long orc_rx_run(orc_rx_t* r, const float* iq, long nsamples,
                 if (orc_deint_push(r->deint, r->cif + r->cfg.subch_start_cu * 64, dtmp)) {
                     orc_msc_deconvolve(&r->cfg.prot, dtmp, obits);
                     orc_dedisperse(obits, 24 * r->cfg.prot.bitrate);
-                    uint8_t fr[3 * 384];
                     orc_pack_bits(obits, flen, fr);
                     if (nmsc + flen <= msc_cap) memcpy(msc + nmsc, fr, flen);
                     nmsc += flen;
@@ -1046,7 +1046,7 @@ long orc_rx_run(orc_rx_t* r, const float* iq, long nsamples,
         else if (r->fine < -ORC_CARRIER_DIFF / 2) { r->coarse -= ORC_CARRIER_DIFF; r->fine += ORC_CARRIER_DIFF; }
     }
 done:
-    free(prsbuf); free(syms); free(nullsym); free(soft); free(env); free(dtmp); free(obits);
+    free(prsbuf); free(syms); free(nullsym); free(soft); free(env); free(dtmp); free(obits); free(fr);
     if (n_fibs) *n_fibs = nfib;
     if (n_msc) *n_msc = nmsc;
     if (n_rs) *n_rs = nrs;

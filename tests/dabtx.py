@@ -176,10 +176,12 @@ def fig0_2(sid, subch_id, ascty=63):
 
 
 class DabTx:
-    """One ensemble with one DAB+ sub-channel (EEP) in CUs [start_cu, start_cu + size)."""
+    """One ensemble with one DAB+ sub-channel (EEP) in CUs [start_cu, start_cu + size); dabplus=False: the sub-channel carries random
+    logical frames instead of superframes (DAB content, any bitrate)."""
 
-    def __init__(self, seed=0xDAB, bitrate=96, profile_a=True, level=3, start_cu=0, subch_id=0, sid=0x1001, amplitude=0.1, period_sf=0):
+    def __init__(self, seed=0xDAB, bitrate=96, profile_a=True, level=3, start_cu=0, subch_id=0, sid=0x1001, amplitude=0.1, period_sf=0, dabplus=True):
         self.period_sf = period_sf          # >0: content repeats every period_sf superframes (= 5*period_sf CIFs): an endless periodic stream
+        self.dabplus = dabplus
         self._sf_cache, self._fill_cache = {}, {}
         self.rng = np.random.default_rng(seed)
         self.bitrate, self.profile_a, self.level = bitrate, profile_a, level
@@ -205,10 +207,13 @@ class DabTx:
 
     # ---- DAB+ superframe
     def superframe(self, bad_au=None, au_starts=None):
-        """one DAB+ superframe (dac_rate=1, sbr=0: 6 AUs); au_starts = the five explicit AU start addresses (else even)"""
+        """one DAB+ superframe (dac_rate=1, sbr=0: 6 AUs); au_starts = the five explicit AU start addresses (else even, as far as the
+        header's 12-bit addresses reach: above 44 RS columns the first five AUs share bytes 11 .. 4095 evenly and the sixth takes the rest)"""
         S = self.S; n_data = 110 * S
         sf = np.zeros(120 * S, np.uint8)
         au = [11] + [11 + (n_data - 11) * i // 6 for i in range(1, 6)] + [n_data]
+        if au[5] > 4095:
+            au = [11] + [11 + (4096 - 11) * i // 6 for i in range(1, 6)] + [n_data]
         if au_starts is not None:
             au = [11] + [int(x) for x in au_starts] + [n_data]
         sf[2] = 0x40
@@ -237,6 +242,8 @@ class DabTx:
 
     def _next_logical(self):
         flen = 3 * self.bitrate
+        if not self.dabplus:
+            return self.rng.integers(0, 256, flen, dtype=np.uint8)
         if len(self._sf_queue) < flen:
             k = len(self.superframes)
             if self.period_sf:

@@ -13,3 +13,10 @@ extern "C" int emul_prot_map(int fic, int bitrate, int short_form, int uep_level
     build_msc_map(*t, p, map);
     return p.in_bits;
 }
+// the energy-dispersal words add_profile and dabb_msc_decode give the decoder for a profile: w [(24 * bitrate + 31) / 32]; returns their number
+extern "C" int emul_prot_prbs_words(int bitrate, uint32_t* w)
+{
+    const int nbits = 24 * bitrate;
+    build_prbs_words(nbits, w);
+    return (nbits + 31) / 32;
+}

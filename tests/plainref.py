@@ -115,6 +115,47 @@ def pack(bits):
     return np.packbits(np.asarray(bits, np.uint8), axis=-1)
 
 
+def eep_blocks(bitrate, profile_a, level):
+    L1, L2, p1, p2 = dabtx.eep_profile(bitrate, profile_a, level)
+    return [(L1, p1), (L2, p2)]
+
+
+def eep_fits(bitrate, profile_a, level):
+    """the EEP profile exists (EEP-A: multiples of 8 kbit/s, EEP-B: of 32) and its sub-channel fits in the 864 CUs of the MSC"""
+    return bitrate > 0 and bitrate % (8 if profile_a else 32) == 0 and dabtx.eep_cu(bitrate, profile_a, level) <= 864
+
+
+def eep_largest(profile_a, level):
+    step = 8 if profile_a else 32
+    return max(b for b in range(step, 2048, step) if eep_fits(b, profile_a, level))
+
+
+# either side of 682 kbit/s (16 384 dispersal bits), where a fixed-length dispersal table used to run out
+EEP_BOUNDARY = [(1, 680), (1, 688), (0, 672), (0, 704)]
+
+
+def eep_wide_profiles():
+    """(profile_a, bitrate, level) from 200 kbit/s up to the largest of every (A/B, level) - EEP 4-A 1728 kbit/s (41 472 bits per logical
+    frame), EEP 4-B 1824 (43 776) - in a stride, with the profiles around 682 kbit/s and the largest ones always in"""
+    out = []
+    for pa, first, stride in ((1, 200, 136), (0, 224, 224)):
+        for lv in (1, 2, 3, 4):
+            brs = set(range(first, eep_largest(pa, lv), stride)) | {b for a, b in EEP_BOUNDARY if a == pa} | {eep_largest(pa, lv)}
+            out += [(pa, b, lv) for b in sorted(brs) if eep_fits(b, pa, lv)]
+    return out
+
+
+def ref_decodes(bitrate):
+    """the reference's Viterbi keeps a logical frame's length in bits as a 16-bit signed integer: above 1365 kbit/s it cannot decode"""
+    return 24 * bitrate <= 32767
+
+
+def eep_wide_soft(profile_a, bitrate, level):
+    """seeded random punctured softbits (-127 .. 127) of one logical frame of the profile"""
+    n_in = int(puncture_mask(eep_blocks(bitrate, profile_a, level)).sum())
+    return np.random.default_rng([profile_a, bitrate, level]).integers(-127, 128, n_in).astype(np.int8)
+
+
 def fib_crc_ok(fib32):
     """32 FIB bytes: CRC-16-CCITT (preset ones, inverted) of the first 30 equals the last two"""
     return dabtx.crc16(fib32[:30]) == (int(fib32[30]) << 8 | int(fib32[31]))

@@ -98,7 +98,7 @@ struct dabb_ctx {
     DevBuf<unsigned long long> d_trace_rec; DevBuf<unsigned int> d_trace_count;      // what `trace` points into
     std::string err; int64_t launches = 0; int osc_mismatches = -1; int osc_patched = 0; std::vector<float2> h_osc;
     HostTables* host = nullptr; DevTables dev{};
-    DevBuf<float2> d_tw_fwd, d_tw_inv, d_prs_ref, d_osc; DevBuf<int16_t> d_invperm, d_fic_map; DevBuf<uint8_t> d_gf_exp, d_gf_log, d_prbs; DevBuf<double2> d_osc_hi;   // what `dev` points into
+    DevBuf<float2> d_tw_fwd, d_tw_inv, d_prs_ref, d_osc; DevBuf<int16_t> d_invperm, d_fic_map; DevBuf<uint8_t> d_gf_exp, d_gf_log; DevBuf<double2> d_osc_hi;   // what `dev` points into
     DevBuf<StreamState> d_state; DevBuf<StepScratch> d_scr; DevBuf<MscSlotState> d_slots;
     DevBuf<int64_t> d_buf_start, d_win, d_prs; DevBuf<int32_t> d_nco_sync, d_nco_frame;
     DevBuf<int32_t> d_active, d_index; DevBuf<float> d_cir, d_cir_work; int search_generic = 0; DevBuf<float2> d_r1, d_null; DevBuf<int32_t> d_snr; DevBuf<float2> d_fc; DevBuf<float> d_lvl;
@@ -199,13 +199,6 @@ void prof_collect(dabb_ctx* ctx)
         if (!found) ctx->prof_acc.push_back({nm, {ms, 1}});
     }
     ctx->prof_used = 0;
-}
-
-void pack_prbs_words(const uint8_t* bits, int nbits, std::vector<uint32_t>& w)
-{
-    // same packing as the decoder output: bit t lands in byte t/8 (MSB first), bytes little-endian in the word
-    w.assign((nbits + 31) / 32, 0);
-    for (int t = 0; t < nbits; t++) if (bits[t]) w[t >> 5] |= 1u << (8 * ((t >> 3) & 3) + 7 - (t & 7));
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -578,7 +571,7 @@ int add_profile(dabb_ctx* ctx, const ProtProfile& prof)
     build_msc_map(*ctx->host, prof, map.data());
     std::vector<uint2> steps; std::vector<uint32_t> soff;
     build_vit_tables_u2(map.data(), pf.nsteps, steps, soff);
-    std::vector<uint32_t> w; pack_prbs_words(ctx->host->prbs, pf.nbits, w);
+    std::vector<uint32_t> w((size_t)(pf.nbits + 31) / 32); build_prbs_words(pf.nbits, w.data());
     int rc;
     if ((rc = dalloc(ctx, pf.d_steptab, steps.size(), false)) || (rc = dalloc(ctx, pf.d_stage_off, soff.size(), false)) || (rc = dalloc(ctx, pf.d_prbs_words, w.size(), false))) return rc;
     VitProfile e{pf.d_steptab, pf.d_stage_off, pf.d_prbs_words, pf.nsteps, pf.nbits};
@@ -659,7 +652,7 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     dabb_ctx* ctx = new dabb_ctx();
     ctx->device = cfg->device; ctx->S = cfg->n_streams; ctx->fft_mode = cfg->fft_mode; ctx->disable_coarse = cfg->disable_coarse; ctx->keep_taps = cfg->keep_taps; ctx->placement = cfg->fft_placement; ctx->freqsync = cfg->freqsync_method;
     ctx->n_slots = cfg->n_subch_slots > 0 ? (cfg->n_subch_slots > DABB_MAX_SUBCH ? DABB_MAX_SUBCH : cfg->n_subch_slots) : 1;
-    ctx->max_cu = cfg->max_subch_cu > 0 ? cfg->max_subch_cu : 144;
+    ctx->max_cu = cfg->max_subch_cu > 0 ? std::min(cfg->max_subch_cu, 864) : 144;     // no sub-channel is larger than the MSC's 864 CUs
     ctx->groups = cfg->ofdm_groups > 0 ? cfg->ofdm_groups : (ctx->S >= 1024 ? 1 : (ctx->S >= 64 ? 5 : 25));
     if (75 % ctx->groups) ctx->groups = 1;
     ctx->nco_fast = cfg->nco_mode == DABB_NCO_FAST;
@@ -684,9 +677,9 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     ctx->fc_pitch = ctx->tail_frames ? OFDM_TAIL_GROUPS : ctx->groups;
     // tables
     auto& tf = ctx->d_tw_fwd; auto& ti = ctx->d_tw_inv; auto& pr = ctx->d_prs_ref; auto& osc = ctx->d_osc; auto& ip = ctx->d_invperm; auto& fm = ctx->d_fic_map;
-    auto& ge = ctx->d_gf_exp; auto& gl = ctx->d_gf_log; auto& pb = ctx->d_prbs;
+    auto& ge = ctx->d_gf_exp; auto& gl = ctx->d_gf_log;
     if ((rc = dalloc(ctx, tf, TwLayout::TOTAL)) || (rc = dalloc(ctx, ti, TwLayout::TOTAL)) || (rc = dalloc(ctx, pr, TU)) || (rc = dalloc(ctx, osc, INPUT_RATE, false)) ||
-        (rc = dalloc(ctx, ip, sizeof ctx->host->invperm / sizeof(int16_t))) || (rc = dalloc(ctx, fm, 3096)) || (rc = dalloc(ctx, ge, 512)) || (rc = dalloc(ctx, gl, 256)) || (rc = dalloc(ctx, pb, sizeof ctx->host->prbs)))
+        (rc = dalloc(ctx, ip, sizeof ctx->host->invperm / sizeof(int16_t))) || (rc = dalloc(ctx, fm, 3096)) || (rc = dalloc(ctx, ge, 512)) || (rc = dalloc(ctx, gl, 256)))
         return fail(rc);
     {
         ctx->h_osc.resize(INPUT_RATE);
@@ -699,11 +692,10 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
         cudaMemcpyAsync(fm, ctx->host->fic_map, sizeof(int16_t) * 3096, cudaMemcpyHostToDevice, ctx->stream);
         cudaMemcpyAsync(ge, ctx->host->gf_exp, 512, cudaMemcpyHostToDevice, ctx->stream);
         cudaMemcpyAsync(gl, ctx->host->gf_log, 256, cudaMemcpyHostToDevice, ctx->stream);
-        cudaMemcpyAsync(pb, ctx->host->prbs, sizeof ctx->host->prbs, cudaMemcpyHostToDevice, ctx->stream);
         if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) { ctx->err = "table upload failed"; return fail(DABB_E_CUDA); }
     }
     ctx->dev.tw_fwd = tf; ctx->dev.tw_inv = ti; ctx->dev.prs_ref = pr; ctx->dev.osc = osc; ctx->dev.invperm = ip; ctx->dev.fic_map = fm;
-    ctx->dev.gf_exp = ge; ctx->dev.gf_log = gl; ctx->dev.prbs = pb;
+    ctx->dev.gf_exp = ge; ctx->dev.gf_log = gl;
     {
         // on-the-fly oscillator: upload the factors, compare against the table for every index on the device, adopt it only when
         // nothing differs (else the kernels keep the table lookups)
@@ -719,7 +711,7 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
         std::vector<float2>().swap(ctx->h_osc);
     }
     {
-        std::vector<uint32_t> w; pack_prbs_words(ctx->host->prbs, 768, w);
+        std::vector<uint32_t> w(768 / 32); build_prbs_words(768, w.data());
         if ((rc = dalloc(ctx, ctx->d_fic_prbs_words, w.size()))) return fail(rc);
         cudaMemcpy(ctx->d_fic_prbs_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice);
         // expansion tables of the decoder kernel for the FIC puncturing (fic-handler.cpp:144-191)
@@ -1342,7 +1334,7 @@ int dabb_msc_decode(dabb_ctx* ctx, const dabb_subchannel* sc, const int8_t* soft
     if (prof.in_bits > frag) { ctx->err = "protection profile needs more bits than the sub-channel holds"; return DABB_E_ARG; }
     std::vector<int16_t> map((size_t)nsteps * 4);
     build_msc_map(*ctx->host, prof, map.data());
-    std::vector<uint32_t> w; pack_prbs_words(ctx->host->prbs, nbits, w);
+    std::vector<uint32_t> w((size_t)(nbits + 31) / 32); build_prbs_words(nbits, w.data());
     DevBuf<uint32_t> d_w;
     int rc;
     if ((rc = dalloc(ctx, d_w, w.size(), false))) return rc;

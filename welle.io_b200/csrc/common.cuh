@@ -22,7 +22,6 @@ struct DevTables {
                                // the reference's own double angle is an ulp off and the factor is the table value itself
     double osc_theta;          // 2 pi / 2 048 000, correctly rounded
     int32_t osc_mode;          // 0: table lookups (a scattered 8-byte gather per sample), 1: on the fly
-    const uint8_t* prbs;       // [9216+] energy-dispersal PRBS bits (fic-handler.cpp:62-71)
     const int16_t* fic_map;    // [3096] mother-code position -> index into the 2304 punctured softbits or -1
     const uint8_t* gf_exp;     // [512]
     const uint8_t* gf_log;     // [256]
@@ -101,7 +100,6 @@ struct HostTables {
     float2 tw_fwd[TwLayout::TOTAL], tw_inv[TwLayout::TOTAL];
     int16_t perm[KC]; int16_t invperm[TU + TU + 192];   // [0, T_u) bin -> logical carrier; [T_u, 2 T_u) bin -> softbit staging index; then the staging slot of each 16-byte chunk
     float2 prs_ref[TU];
-    uint8_t prbs[16384];
     int16_t fic_map[3096];
     uint8_t gf_exp[512], gf_log[256];
     int8_t pcodes[24][32];
@@ -117,5 +115,7 @@ struct ProtProfile { int bitrate; int nblk; int L[4]; int PI[4]; int in_bits; };
 int make_prot_profile(int bitrate, int short_form, int uep_level, int eep_profile_a, int eep_level, ProtProfile& out);
 // mother-code map: for each of 4*(24*bitrate+6) positions the index into the punctured input (saturating at 32767) or -1
 void build_msc_map(const HostTables& t, const ProtProfile& p, int16_t* map);
+// energy-dispersal words of an nbits-bit block ((nbits + 31) / 32 of them), packed like the decoder output
+void build_prbs_words(int nbits, uint32_t* w);
 
 } // namespace dabb

@@ -104,15 +104,6 @@ void build_host_tables(HostTables& t)
         p = prs_phi(-i);
         t.prs_ref[TU - i] = make_float2(cosf(p), sinf(p));
     }
-    // PRBS x^9 + x^5 + 1, all-ones preset (fic-handler.cpp:62-71, energy_dispersal.h:40-49)
-    {
-        unsigned reg = 0x1FF;
-        for (size_t i = 0; i < sizeof t.prbs; i++) {
-            unsigned b = ((reg >> 8) ^ (reg >> 4)) & 1;
-            reg = ((reg << 1) | b) & 0x1FF;
-            t.prbs[i] = (uint8_t)b;
-        }
-    }
     // puncturing vectors PI_1..PI_24 (protTables.cpp:25-51): groups of 4 start as 1000; bits are switched on
     // group by group in the order 0,4,2,6,1,5,3,7, one column per eight steps
     {
@@ -213,6 +204,19 @@ void build_msc_map(const HostTables& t, const ProtProfile& p, int16_t* map)
     for (int k = 0; k < p.nblk; k++)
         for (int i = 0; i < p.L[k] * 128; i++, pos++) map[pos] = t.pcodes[p.PI[k] - 1][i & 31] ? next() : (int16_t)-1;
     for (int i = 0; i < 24; i++, pos++) map[pos] = ((i & 3) < 2) ? next() : (int16_t)-1;
+}
+
+void build_prbs_words(int nbits, uint32_t* w)
+{
+    // PRBS x^9 + x^5 + 1, all-ones preset (fic-handler.cpp:62-71, energy_dispersal.h:40-49), run for the block's own length: an MSC
+    // logical frame has up to 24 x 1824 bits.  Packed like the decoder output: bit t in byte t/8 (MSB first), bytes little-endian in the word
+    memset(w, 0, sizeof(uint32_t) * (size_t)((nbits + 31) / 32));
+    unsigned reg = 0x1FF;
+    for (int t = 0; t < nbits; t++) {
+        const unsigned b = ((reg >> 8) ^ (reg >> 4)) & 1;
+        reg = ((reg << 1) | b) & 0x1FF;
+        if (b) w[t >> 5] |= 1u << (8 * ((t >> 3) & 3) + 7 - (t & 7));
+    }
 }
 
 } // namespace dabb
