@@ -81,8 +81,22 @@ typedef struct {
     int32_t freqsync_method;    /* DABB_FREQSYNC_* */
     int32_t decode_tii;         /* RadioReceiverOptions::decodeTII: analyse the transmitter identification of every decoded frame on the device
                                    (tap 9); with keep_taps, also produce tap 4 (the two spectra TIIDecoder starts from) */
-    int32_t reserved[4];
+    int32_t count_bit_errors;   /* count the channel bit errors of the FIC and of every decoded sub-channel codeword on the device (tap 10) */
+    int32_t reserved[3];
 } dabb_options;
+
+/* Channel bit errors of one stream in one step: tap 10, while dabb_options.count_bit_errors is set.  Per codeword (a FIC block of 768
+ * bits, or a logical frame of 24 * bitrate bits) the decoded bits before energy dispersal (the output bytes MSB first, XOR the PRBS; 6
+ * zero tail bits) are re-encoded with the K=7 rate-1/4 mother code and punctured like the codeword's protection (FIC: 21 x PI_16,
+ * 3 x PI_15; EEP / UEP: the profile's blocks; both with the tail).  The k-th transmitted bit is the k-th softbit the decoder read
+ * (softbits past the profile's own length are not counted).  A softbit 0 is an erasure; otherwise s > 0 decides 1 and s < 0 decides 0,
+ * and an error is a decision that differs from the re-encoded bit.  bits counts the transmitted positions, erasures included:
+ * channel BER = errors / (bits - erasures).  The FIC counts cover the 4 codewords of a frame with status DABB_FRAME_DECODED; subch[k]
+ * covers the logical frames the step delivered in slot k (codewords == n_logical[k]).  Everything else is zero. */
+typedef struct {
+    int32_t fic_bits, fic_errors, fic_erasures, reserved;
+    struct { int32_t codewords, bits, errors, erasures; } subch[DABB_MAX_SUBCH];
+} dabb_ber_result;
 
 /* Transmitter identification (TIIDecoder, backend/tii-decoder.cpp:236-383) of one stream in one step: tap 9.  Every decoded frame is
  * analysed while dabb_options.decode_tii is set; each (comb, pattern) combination found in a frame accumulates its phase-error table over
@@ -238,7 +252,9 @@ int dabb_profile_read(dabb_ctx* ctx, char* json_out, size_t cap);
  *   7 = logical frames uint8 [n_streams][DABB_MAX_SUBCH][4][stride], the layout of dabb_io.msc; stride = bytes / (n_streams * DABB_MAX_SUBCH * 4)
  *   8 = DAB+ superframes uint8 [n_streams][DABB_MAX_SUBCH][stride], the layout of dabb_io.sf; stride = bytes / (n_streams * DABB_MAX_SUBCH)
  *   9 = dabb_tii_result [n_streams] of the last step (all zero when that step ran with decode_tii off); DABB_E_STATE until
- *       dabb_options.decode_tii has been set once */
+ *       dabb_options.decode_tii has been set once
+ *  10 = dabb_ber_result [n_streams] of the last step (all zero when that step ran with count_bit_errors off); DABB_E_STATE until
+ *       dabb_options.count_bit_errors has been set once */
 int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes);
 
 /* ---------------------------------------------------------------------------------------------------------

@@ -94,6 +94,9 @@ struct dabb_ctx {
     // combinations and their phase-error sums, the step's analyses, the tie-order tables and the step's records (tap 9)
     DevBuf<float2> d_tii_null; DevBuf<dabb_tii::StreamHdr> d_tii_hdr; DevBuf<dabb_tii::Job> d_tii_jobs; DevBuf<int32_t> d_tii_njobs;
     DevBuf<uint32_t> d_tii_sums; DevBuf<uint16_t> d_tii_rank; DevBuf<dabb_tii_result> d_tii_res;
+    // channel bit-error count (ber.cu), allocated when count_bit_errors is first set: the puncturing of every protection profile and of the
+    // FIC as the count reads it ([DABB_MAX_PROFILES] then the FIC) and the step's records (tap 10)
+    int count_ber = 0; dabb_ber::Profile h_ber_fic{}; DevBuf<dabb_ber::Profile> d_ber_prof; DevBuf<dabb_ber_result> d_ber_res;
     TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0;
     DevBuf<unsigned long long> d_trace_rec; DevBuf<unsigned int> d_trace_count;      // what `trace` points into
     std::string err; int64_t launches = 0; int osc_mismatches = -1; int osc_patched = 0; std::vector<float2> h_osc;
@@ -109,6 +112,7 @@ struct dabb_ctx {
     struct Profile {
         ProtProfile prof{}; int nsteps = 0, nbits = 0, flen = 0, flen_pad = 0;
         DevBuf<uint2> d_steptab; DevBuf<uint32_t> d_stage_off, d_prbs_words;
+        dabb_ber::Profile ber{};        // its puncturing as the bit-error count reads it (d_ber_prof)
     };
     std::vector<Profile> profiles; DevBuf<VitProfile> d_profiles;
     // per slot: the buffers of the streams that decode a sub-channel in it.  Rows of d_logical / d_window / d_sf are flen_pad bytes
@@ -579,6 +583,8 @@ int add_profile(dabb_ctx* ctx, const ProtProfile& prof)
     CK(cudaMemcpyAsync(pf.d_stage_off, soff.data(), soff.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(pf.d_prbs_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_profiles + ctx->profiles.size(), &e, sizeof e, cudaMemcpyHostToDevice, ctx->stream));
+    build_ber_profile(*ctx->host, prof.nblk, prof.L, prof.PI, pf.nbits, pf.ber); pf.ber.prbs = pf.d_prbs_words;
+    if (ctx->d_ber_prof) CK(cudaMemcpyAsync(ctx->d_ber_prof + ctx->profiles.size(), &pf.ber, sizeof pf.ber, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->profiles.push_back(std::move(pf));
     return DABB_OK;
@@ -714,6 +720,8 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
         std::vector<uint32_t> w(768 / 32); build_prbs_words(768, w.data());
         if ((rc = dalloc(ctx, ctx->d_fic_prbs_words, w.size()))) return fail(rc);
         cudaMemcpy(ctx->d_fic_prbs_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice);
+        const int fic_L[2] = {21, 3}, fic_PI[2] = {16, 15};
+        build_ber_profile(*ctx->host, 2, fic_L, fic_PI, 768, ctx->h_ber_fic); ctx->h_ber_fic.prbs = ctx->d_fic_prbs_words;
         // expansion tables of the decoder kernel for the FIC puncturing (fic-handler.cpp:144-191)
         std::vector<uint2> steps; std::vector<uint32_t> soff;
         build_vit_tables_u2(ctx->host->fic_map, 774, steps, soff);
@@ -1019,6 +1027,17 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         if ((rc = check_launch(ctx, "superframe_kernel"))) return rc;
     }
     if (!serial) CK(cudaStreamWaitEvent(B, ctx->ev_fic, 0));
+    // the channel bit errors of the step's FIC and logical frames, while its FIBs, fragments and logical frames are all in place
+    if (ctx->count_ber) {
+        BerParams bp{}; bp.soft = d_soft; bp.soft_stride = DABB_SOFT_PER_FRAME; bp.fibs = ctx->d_fibs; bp.active = d_active; bp.slots = ctx->d_slots; bp.n_slots = ctx->n_slots;
+        for (int k = 0; k < ctx->n_slots; k++) {
+            const auto& sl = ctx->slot[k];
+            if (sl.configured) bp.slot[k] = BerSlot{sl.d_frag, sl.frag_pitch, sl.d_valid, sl.d_logical, sl.flen_pad};
+        }
+        bp.profiles = ctx->d_ber_prof; bp.fic_profile = DABB_MAX_PROFILES; bp.res = ctx->d_ber_res.get(); bp.n_streams = S;
+        launch_ber(bp, B);
+        if ((rc = check_launch(ctx, "ber_kernel"))) return rc;
+    } else if (ctx->d_ber_res) CK(cudaMemsetAsync(ctx->d_ber_res, 0, sizeof(dabb_ber_result) * S, B));     // tap 10: nothing counted in this step
     CK(cudaMemcpyAsync((void*)ctx->d_info_tab, h_info, sizeof(void*) * DABB_MAX_SUBCH, cudaMemcpyHostToDevice, B));
     finalize_kernel<<<gb, tb, 0, B>>>(scr, ctx->d_slots, ctx->n_slots, S, ctx->d_fic_ratio, d_snr, ctx->d_crc, ctx->d_info_tab, ctx->d_results);
     if ((rc = check_launch(ctx, "finalize_kernel"))) return rc;
@@ -1156,6 +1175,10 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
         if (!ctx->d_tii_res) { ctx->err = "tap 9 needs dabb_options.decode_tii to have been set"; return DABB_E_STATE; }
         const size_t n = sizeof(dabb_tii_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_tii_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
     }
+    if (what == 10) {
+        if (!ctx->d_ber_res) { ctx->err = "tap 10 needs dabb_options.count_bit_errors to have been set"; return DABB_E_STATE; }
+        const size_t n = sizeof(dabb_ber_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_ber_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
+    }
     if (what == 4 && ctx->d_tii && ctx->d_null && ctx->decode_tii) { const size_t n = (size_t)ctx->S * 2 * TU * 8; CK(cudaMemcpy(host_out, ctx->d_tii, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 3 && ctx->d_null) { const size_t n = (size_t)ctx->S * TNULL * 8; CK(cudaMemcpy(host_out, ctx->d_null, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 5) { const size_t n = sizeof(dabb_frame_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_results, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
@@ -1259,7 +1282,18 @@ int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
         if ((rc = dalloc(ctx, ctx->d_tii_res, S))) return rc;      // last: it marks the analysis as available
         CK(cudaStreamSynchronize(ctx->stream));
     }
+    if (opt->count_bit_errors && !ctx->d_ber_res) {     // first use of the bit-error count: the puncturing of every profile so far and of the FIC
+        cudaSetDevice(ctx->device);
+        sync_all(ctx);
+        int rc;
+        if ((rc = dalloc(ctx, ctx->d_ber_prof, DABB_MAX_PROFILES + 1))) return rc;
+        for (size_t i = 0; i < ctx->profiles.size(); i++) CK(cudaMemcpyAsync(ctx->d_ber_prof + i, &ctx->profiles[i].ber, sizeof(dabb_ber::Profile), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->d_ber_prof + DABB_MAX_PROFILES, &ctx->h_ber_fic, sizeof(dabb_ber::Profile), cudaMemcpyHostToDevice, ctx->stream));
+        if ((rc = dalloc(ctx, ctx->d_ber_res, (size_t)ctx->S))) { ctx->d_ber_prof.reset(); return rc; }      // last: it marks the count as available
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
     ctx->disable_coarse = opt->disable_coarse != 0; ctx->placement = opt->fft_placement; ctx->freqsync = opt->freqsync_method; ctx->decode_tii = opt->decode_tii != 0;
+    ctx->count_ber = opt->count_bit_errors != 0;
     return DABB_OK;
 }
 

@@ -5,6 +5,7 @@
 #include <string>
 #include "ofdm_core.cuh"
 #include "tii_core.cuh"
+#include "ber_core.cuh"
 
 namespace dabb {
 
@@ -117,5 +118,8 @@ int make_prot_profile(int bitrate, int short_form, int uep_level, int eep_profil
 void build_msc_map(const HostTables& t, const ProtProfile& p, int16_t* map);
 // energy-dispersal words of an nbits-bit block ((nbits + 31) / 32 of them), packed like the decoder output
 void build_prbs_words(int nbits, uint32_t* w);
+// the puncturing of nbits-bit codewords with blocks (L[k], PI[k]) and the tail, as the bit-error count reads it (ber_core.cuh); the
+// dispersal words (Profile::prbs) are the caller's
+void build_ber_profile(const HostTables& t, int nblk, const int* L, const int* PI, int nbits, dabb_ber::Profile& out);
 
 } // namespace dabb

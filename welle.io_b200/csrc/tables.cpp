@@ -206,6 +206,15 @@ void build_msc_map(const HostTables& t, const ProtProfile& p, int16_t* map)
     for (int i = 0; i < 24; i++, pos++) map[pos] = ((i & 3) < 2) ? next() : (int16_t)-1;
 }
 
+void build_ber_profile(const HostTables& t, int nblk, const int* L, const int* PI, int nbits, dabb_ber::Profile& out)
+{
+    // the same vectors build_msc_map and the FIC map expand (bit i of a mask = entry i of PI_n)
+    uint32_t mask[4] = {0, 0, 0, 0};
+    for (int k = 0; k < nblk; k++)
+        if (L[k] > 0) for (int i = 0; i < 32; i++) mask[k] |= (uint32_t)(t.pcodes[PI[k] - 1][i] != 0) << i;
+    dabb_ber::build_profile(nblk, L, mask, nbits, out);
+}
+
 void build_prbs_words(int nbits, uint32_t* w)
 {
     // PRBS x^9 + x^5 + 1, all-ones preset (fic-handler.cpp:62-71, energy_dispersal.h:40-49), run for the block's own length: an MSC

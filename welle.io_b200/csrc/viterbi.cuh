@@ -82,4 +82,24 @@ void launch_superframe(const SuperframeParams& p, cudaStream_t st);
 // stateless: RS + sync check + AU CRCs on n superframes in place; info[n][4]
 void launch_rs_superframes(uint8_t* sf, int n, int sf_len, int32_t* info, const uint8_t* gf_exp, const uint8_t* gf_log, cudaStream_t st);
 
+// ---- ber.cu ----
+// one sub-channel slot as the bit-error count reads it; frag == nullptr: the slot is not configured
+struct BerSlot {
+    const int8_t* frag; int64_t frag_pitch;            // [n_streams*4][frag_pitch] the step's fragments (MscPrepParams::frag_out)
+    const int32_t* valid;                              // [n_streams*4] codewords the step decoded
+    const uint8_t* logical; int64_t logical_stride;    // [n_streams*4][stride] their logical frames
+};
+struct BerParams {
+    const int8_t* soft; int64_t soft_stride;           // FIC codeword (s, b) = softbits [2304 b, 2304 b + 2304) of frame s
+    const uint8_t* fibs;                               // [n_streams*4][96] decoded FIC blocks
+    const int32_t* active;                             // [n_streams] 1 = the frame was decoded
+    const MscSlotState* slots; int n_slots;
+    BerSlot slot[4];                                   // DABB_MAX_SUBCH
+    const dabb_ber::Profile* profiles;                 // [DABB_MAX_PROFILES + 1]: the context's protection profiles, then the FIC
+    int fic_profile;                                   // index of the FIC's entry
+    void* res;                                         // [n_streams] dabb_ber_result
+    int n_streams;
+};
+void launch_ber(const BerParams& p, cudaStream_t st);
+
 } // namespace dabb

@@ -32,7 +32,7 @@ class Config(C.Structure):
 
 
 class Options(C.Structure):
-    _fields_ = [("disable_coarse", C.c_int32), ("fft_placement", C.c_int32), ("freqsync_method", C.c_int32), ("decode_tii", C.c_int32), ("reserved", C.c_int32 * 4)]
+    _fields_ = [("disable_coarse", C.c_int32), ("fft_placement", C.c_int32), ("freqsync_method", C.c_int32), ("decode_tii", C.c_int32), ("count_bit_errors", C.c_int32), ("reserved", C.c_int32 * 3)]
 
 
 PLACEMENT_THRESHOLD_BEFORE_PEAK, PLACEMENT_STRONGEST_PEAK, PLACEMENT_EARLIEST_PEAK_WITH_BINNING = 0, 1, 2
@@ -66,6 +66,10 @@ TII_MAX = 9
 TII_DTYPE = np.dtype([("count", "<i4"), ("evicted", "<i4"), ("skipped", "<i4"), ("reserved", "<i4"),
                       ("m", [("comb", "<i4"), ("pattern", "<i4"), ("delay_samples", "<i4"), ("error", "<f4")], (TII_MAX,))])
 assert TII_DTYPE.itemsize == 16 + 16 * TII_MAX
+# dabb_ber_result: one stream's channel bit errors of one step (tap 10)
+BER_DTYPE = np.dtype([("fic_bits", "<i4"), ("fic_errors", "<i4"), ("fic_erasures", "<i4"), ("reserved", "<i4"),
+                      ("subch", [("codewords", "<i4"), ("bits", "<i4"), ("errors", "<i4"), ("erasures", "<i4")], (MAX_SUBCH,))])
+assert BER_DTYPE.itemsize == 80
 
 
 class IO(C.Structure):
@@ -304,14 +308,16 @@ class Context:
         self._ck(self.lib.dabb_get_info(self.h, int(what), C.byref(v)))
         return v.value
 
-    def set_options(self, disable_coarse=True, fft_placement=0, freqsync_method=0, decode_tii=False):
+    def set_options(self, disable_coarse=True, fft_placement=0, freqsync_method=0, decode_tii=False, count_bit_errors=False):
         o = Options(); o.disable_coarse, o.fft_placement, o.freqsync_method, o.decode_tii = int(disable_coarse), int(fft_placement), int(freqsync_method), int(decode_tii)
+        o.count_bit_errors = int(count_bit_errors)
         self._ck(self.lib.dabb_set_options(self.h, C.byref(o)))
 
     def read_tap(self, what, stride=0):
         """0 softbits, 1 CIR, 2 constellation points (75 x 16 per stream), 3 null symbol (2656 samples, NCO applied),
         4 TII spectra (PRS, null symbol), 5 frame results, 6 FIBs, 7 logical frames [S, MAX_SUBCH, 4, stride] and 8 superframes
-        [S, MAX_SUBCH, stride] of the last step (also after process_async), 9 TII measurements (TII_DTYPE per stream)"""
+        [S, MAX_SUBCH, stride] of the last step (also after process_async), 9 TII measurements (TII_DTYPE per stream), 10 channel bit
+        errors (BER_DTYPE per stream)"""
         if what == 7:
             out = np.zeros((self.n_streams, MAX_SUBCH, 4, stride), np.uint8)
         elif what == 8:
@@ -330,6 +336,8 @@ class Context:
             out = np.zeros((self.n_streams, 2, 2048), np.complex64)
         elif what == 9:
             out = np.zeros(self.n_streams, TII_DTYPE)
+        elif what == 10:
+            out = np.zeros(self.n_streams, BER_DTYPE)
         else:
             out = np.zeros((self.n_streams, TU), np.float32)
         self._ck(self.lib.dabb_read_tap(self.h, what, _vp(out), C.c_size_t(out.nbytes)))

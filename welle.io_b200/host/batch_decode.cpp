@@ -1,7 +1,7 @@
 /*
  * batch_decode.cpp — native batch driver over the C ABI: decodes many RAW IQ recordings at once, one stream per file, on one GPU.
  *
- *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] --out DIR file1 [file2 ...]
+ *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] --out DIR file1 [file2 ...]
  *
  * What `welle-cli -f FILE -D` does for one recording (welle-cli.cpp:215-235,612-707: dump the FIC, tune to the first audio
  * service, dump its logical frames) done for all files in lock-step: every iteration hands each stream's next window of samples
@@ -13,6 +13,9 @@
  *
  * --tii: transmitter identification of every decoded frame, analysed on the device (dabb_options.decode_tii, tap 9); each measurement
  * goes to DIR/<name>.tii as one line "comb pattern delay_samples error", the format of glue_test's .tii (onTIIMeasurement).
+ *
+ * --ber: channel bit errors counted on the device (dabb_options.count_bit_errors, tap 10); every decoded frame adds one line
+ * "fic_bits fic_errors fic_erasures codewords bits errors erasures" to DIR/<name>.ber, the last four for the service's slot (0).
  *
  * Sample formats are the RAW-file formats of CRAWFile (input/raw_file.cpp:324-366); they are shipped as they are and converted on
  * the device.
@@ -32,7 +35,7 @@
 namespace {
 
 struct Stream {
-    std::string path, name; FILE* in = nullptr; FILE* fic = nullptr; FILE* msc = nullptr; FILE* rs = nullptr; FILE* tii = nullptr;
+    std::string path, name; FILE* in = nullptr; FILE* fic = nullptr; FILE* msc = nullptr; FILE* rs = nullptr; FILE* tii = nullptr; FILE* ber = nullptr;
     int64_t buf_start = 0, have = 0, pos = 0, acq_need = 0;      /* logical sample indices; `have` samples are buffered from buf_start */
     bool tracking = false, eof = false, done = false;
     std::unique_ptr<dabb_host::FigDb> db{new dabb_host::FigDb()};
@@ -46,7 +49,7 @@ int bytes_per_sample(int fmt) { return fmt == DABB_IQ_CF32 ? 8 : (fmt == DABB_IQ
 
 int main(int argc, char** argv)
 {
-    int fmt = DABB_IQ_CF32, device = 0; bool coarse = false, tii = false; std::string out;
+    int fmt = DABB_IQ_CF32, device = 0; bool coarse = false, tii = false, ber = false; std::string out;
     std::vector<std::string> files;
     for (int i = 1; i < argc; i++) {
         const std::string a = argv[i];
@@ -59,9 +62,10 @@ int main(int argc, char** argv)
         else if (a == "--out" && i + 1 < argc) out = argv[++i];
         else if (a == "--coarse") coarse = true;
         else if (a == "--tii") tii = true;
+        else if (a == "--ber") ber = true;
         else files.push_back(a);
     }
-    if (out.empty() || files.empty()) { fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] --out DIR file...\n"); return 2; }
+    if (out.empty() || files.empty()) { fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] --out DIR file...\n"); return 2; }
 
     const int S = (int)files.size();
     const int64_t TF = DABB_TF, W = 6 * TF;                       /* per-stream window capacity in samples */
@@ -73,9 +77,9 @@ int main(int argc, char** argv)
     cfg.disable_coarse = coarse ? 0 : 1; cfg.n_subch_slots = DABB_MAX_SUBCH; cfg.max_subch_cu = 416;
     dabb_ctx* ctx = nullptr;
     if (dabb_create(&cfg, &ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return 1; }
-    if (tii) {
+    if (tii || ber) {
         dabb_options op; memset(&op, 0, sizeof op);
-        op.disable_coarse = cfg.disable_coarse; op.decode_tii = 1;
+        op.disable_coarse = cfg.disable_coarse; op.decode_tii = tii; op.count_bit_errors = ber;
         if (dabb_set_options(ctx, &op) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
     }
 
@@ -89,7 +93,8 @@ int main(int argc, char** argv)
         if (!z.in) { fprintf(stderr, "batch_decode: cannot open %s\n", z.path.c_str()); return 1; }
         z.fic = fopen((out + "/" + z.name + ".fic").c_str(), "wb"); z.msc = fopen((out + "/" + z.name + ".msc").c_str(), "wb"); z.rs = fopen((out + "/" + z.name + ".rs").c_str(), "w");
         if (tii) z.tii = fopen((out + "/" + z.name + ".tii").c_str(), "w");
-        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
+        if (ber) z.ber = fopen((out + "/" + z.name + ".ber").c_str(), "w");
+        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii) || (ber && !z.ber)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
         z.acq_need = 3 * TF;
     }
     dabb_stream_reset(ctx, 0, S, 0);
@@ -99,6 +104,7 @@ int main(int argc, char** argv)
     std::vector<dabb_frame_result> res((size_t)S);
     std::vector<uint8_t> fibs((size_t)S * 12 * 32), msc((size_t)S * DABB_MAX_SUBCH * 4 * 1152), sf((size_t)S * DABB_MAX_SUBCH * 5760);
     std::vector<dabb_tii_result> tres(tii ? (size_t)S : 0);
+    std::vector<dabb_ber_result> bres(ber ? (size_t)S : 0);
 
     int active = S;
     while (active > 0) {
@@ -143,6 +149,7 @@ int main(int argc, char** argv)
         io.results = res.data(); io.fibs = fibs.data(); io.msc = msc.data(); io.msc_stride = 1152; io.sf = sf.data(); io.sf_stride = 5760; io.iq_format = fmt;
         if (dabb_process(ctx, &io) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
         if (tii && dabb_read_tap(ctx, 9, tres.data(), tres.size() * sizeof(dabb_tii_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
+        if (ber && dabb_read_tap(ctx, 10, bres.data(), bres.size() * sizeof(dabb_ber_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
 
         /* 2. per-stream results */
         for (int s = 0; s < S; s++) {
@@ -165,6 +172,10 @@ int main(int argc, char** argv)
                 continue;
             }
             z.tracking = true; z.acq_need = 3 * TF; z.frames++;
+            if (ber) {
+                const dabb_ber_result& b = bres[(size_t)s];
+                fprintf(z.ber, "%d %d %d %d %d %d %d\n", b.fic_bits, b.fic_errors, b.fic_erasures, b.subch[0].codewords, b.subch[0].bits, b.subch[0].errors, b.subch[0].erasures);
+            }
             for (int f = 0; f < 12; f++) {
                 const uint8_t* fb = fibs.data() + ((size_t)s * 12 + (size_t)f) * 32;
                 const uint8_t ok = (r.fib_crc_mask >> f) & 1;
@@ -197,7 +208,7 @@ int main(int argc, char** argv)
     }
     for (auto& z : st) {
         printf("%s frames=%ld fibs=%ld fib_crc_ok=%ld service=0x%X bitrate=%d logical_frames=%ld\n", z.name.c_str(), z.frames, z.fibs, z.fibs_ok, z.sid, z.bitrate, z.logical);
-        fclose(z.in); fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii);
+        fclose(z.in); fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii); if (z.ber) fclose(z.ber);
     }
     dabb_destroy(ctx);
     return 0;
