@@ -258,6 +258,61 @@ int dabb_profile_read(dabb_ctx* ctx, char* json_out, size_t cap);
 int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Wideband channelizer: turns recordings at other sample rates, tuned between ensembles or holding several of them, into the
+ * 2 048 000 samples/s streams dabb_process decodes.
+ * replaces: none.  The reference's only rate conversion is the Airspy driver's 2:1 average of neighbouring samples
+ * (input/airspy_sdr.cpp:188-209); its input layer hands the backend 2.048 Msps only.
+ *
+ * A channelizer belongs to a context.  It reads n_inputs wideband inputs at a common rate R Hz (an integer) in one DABB_IQ_* format
+ * (converted exactly like convert_iq_kernel / CRAWFile::convertSamples) and produces n_channels channels; channel c reads input
+ * input_of_channel[c] and is centred at offset_hz[c].  Accepted: 2 048 000 <= R <= 64 000 000 with 2 048 000 / R = L / M in lowest
+ * terms and L <= 1024 (2.048, 2.4, 2.5, 3, 4.096, 6, 8, 8.192, 10, 20, 61.44 Msps and more), |offset_hz| + 768 000 <= R / 2,
+ * 1 <= n_channels <= 4096; a rate outside this is DABB_E_UNSUPPORTED, anything else malformed DABB_E_ARG.
+ *
+ * Filter: one Kaiser-windowed-sinc prototype h of L*T taps at rate L*R, cutoff 856 000 Hz (midway between the 768 kHz edge of the
+ * 1536 carriers and the 944 kHz edge of the neighbouring ensemble), beta = 0.1102 * (72 - 8.7), T = ceil((72 - 7.95) /
+ * (14.36 * 176 000 / R)) + 1 taps per branch; designed in double, scaled so that the taps sum to L, rounded to float.  At the rates
+ * listed above it has at most 0.005 dB ripple for |f| <= 768 kHz and at least 71 dB attenuation for |f| >= 944 kHz.
+ *
+ * Output m of channel c is the absolute sample index m on that channel's 2.048 Msps axis.  With n_m = floor(m M / L),
+ * p_m = (m M) mod L and x the channel's input:
+ *     y[m] = sum_{j=0}^{T-1} h[p_m + j L] x[n_m - j] exp(-2 pi i k(n_m - j) / R),   k(n) = (offset_hz * n) mod R in exact integers
+ * so an output depends on m and the input samples [n_m - T + 1, n_m] only.  The channelizer keeps no state between calls: cutting a
+ * run into calls of any size gives the same samples bit for bit, and a stream that re-acquires simply asks for another range.
+ * Every output is within 1e-5 of rms(y) (rms error) and 1e-4 (largest error) of the same sum in exact arithmetic. */
+typedef struct dabb_chan dabb_chan;
+typedef struct {
+    int64_t rate_hz;                    /* R */
+    int32_t iq_format;                  /* DABB_IQ_* of the inputs */
+    int32_t n_inputs;
+    int32_t n_channels;
+    int32_t reserved;
+    const int32_t* input_of_channel;    /* [n_channels] host array, 0 .. n_inputs - 1 */
+    const int64_t* offset_hz;           /* [n_channels] host array */
+} dabb_chan_config;
+/* creates a channelizer of ctx (designs its filter and uploads it).  A context that never creates one allocates nothing for it.
+ * Destroy every channelizer of a context before the context. */
+int dabb_chan_create(dabb_ctx* ctx, const dabb_chan_config* cfg, dabb_chan** out);
+void dabb_chan_destroy(dabb_chan* ch);   /* NULL is a no-op; waits for the context's work */
+/* the input span [*in_first, *in_end) (absolute input indices) that outputs [out_start, out_start + out_len) of any channel read:
+ * in_first = n_{out_start} - T + 1, in_end = n_{out_start + out_len - 1} + 1.  out_start >= 0, out_len >= 1 */
+int dabb_chan_input_range(const dabb_chan* ch, int64_t out_start, int64_t out_len, int64_t* in_first, int64_t* in_end);
+/* One channelizer call.
+ *   in            input i at in + i * in_stride samples of the configured format; host (in_is_host = 1, copied inside the call) or device
+ *   in_start[i]   absolute index of input i's first sample (host array, n_inputs entries); every buffer holds in_len samples
+ *   out           device float2 [n_channels][out_stride]: row c receives outputs [out_start[c], out_start[c] + out_len) of channel c
+ *   out_start[c]  host array, n_channels entries, >= 0; out_start[c] + out_len <= 2^45
+ * The work is enqueued on the context's main stream, so a following dabb_process / dabb_process_async on the same context reads `out`
+ * as a device iq (iq_is_host = 0, stride_samples = out_stride, buf_start[s] = out_start[s]).  Arguments are checked before anything is
+ * enqueued: a NULL pointer, out_len < 1, a stride below its length, or a channel whose input span (dabb_chan_input_range) does not
+ * lie inside its buffer returns DABB_E_ARG and writes nothing. */
+typedef struct {
+    const void* in; int32_t in_is_host; int64_t in_stride; const int64_t* in_start; int64_t in_len;
+    float* out; int64_t out_stride; const int64_t* out_start; int64_t out_len;
+} dabb_chan_io;
+int dabb_channelize(dabb_chan* ch, const dabb_chan_io* io);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Stage-level entry points (stateless).  Pointers are DEVICE pointers unless named host_*.
  * ------------------------------------------------------------------------------------------------------- */
 

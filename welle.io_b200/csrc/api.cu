@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstring>
 #include <algorithm>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -450,24 +451,14 @@ void sync_all(dabb_ctx* ctx)
     if (ctx->streamC) cudaStreamSynchronize(ctx->streamC);
 }
 
-// raw file formats -> cf32, value for value like CRAWFile::convertSamples (input/raw_file.cpp:336-363): u8 (b-128)/128,
-// s8 b/128, "s16le"/"s16be" unscaled with the byte order the reference applies to each name
+// raw file formats -> cf32, value for value like CRAWFile::convertSamples (dabb_channel::raw_sample, shared with the channelizer)
 __global__ void convert_iq_kernel(const uint8_t* __restrict__ raw, int64_t raw_stride_samples, int fmt, float2* __restrict__ out, int64_t out_stride, int64_t len, int S)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int s = blockIdx.y;
     if (i >= len || s >= S) return;
-    float re, im;
-    if (fmt == DABB_IQ_U8) { const uchar2 b = reinterpret_cast<const uchar2*>(raw)[(int64_t)s * raw_stride_samples + i]; re = (float)((int)b.x - 128) / 128.0f; im = (float)((int)b.y - 128) / 128.0f; }
-    else if (fmt == DABB_IQ_S8) { const char2 b = reinterpret_cast<const char2*>(raw)[(int64_t)s * raw_stride_samples + i]; re = (float)b.x / 128.0f; im = (float)b.y / 128.0f; }
-    else {
-        const uchar4 b = reinterpret_cast<const uchar4*>(raw)[(int64_t)s * raw_stride_samples + i];
-        int16_t I, Q;
-        if (fmt == DABB_IQ_S16LE) { I = (int16_t)((b.x << 8) | b.y); Q = (int16_t)((b.z << 8) | b.w); }
-        else { I = (int16_t)((b.y << 8) | b.x); Q = (int16_t)((b.w << 8) | b.z); }
-        re = (float)I; im = (float)Q;
-    }
-    out[(int64_t)s * out_stride + i] = make_float2(re, im);
+    const dabb_channel::cf v = dabb_channel::raw_sample(raw, (int64_t)s * raw_stride_samples + i, fmt);
+    out[(int64_t)s * out_stride + i] = make_float2(v.x, v.y);
 }
 
 // makes b hold at least n elements, without keeping its contents; the device finishes with the old buffer first
@@ -478,7 +469,7 @@ template <typename T> int grow(dabb_ctx* ctx, DevBuf<T>& b, size_t n)
     return alloc(ctx, b, n);
 }
 
-size_t bytes_per_sample(int fmt) { return fmt == DABB_IQ_CF32 ? 8 : ((fmt == DABB_IQ_U8 || fmt == DABB_IQ_S8) ? 2 : 4); }
+using dabb_channel::bytes_per_sample;
 
 // ---- step outputs ---------------------------------------------------------------------------------------------------------------
 // Every way a step's outputs reach the caller (dabb_process, dabb_submit + dabb_collect, taps 7 / 8) runs the same three routines:
@@ -907,7 +898,7 @@ int dabb_process_async(dabb_ctx* ctx, const dabb_io* io)
     const int fmt = io->iq_format;
     if (fmt < 0 || fmt > DABB_IQ_S16BE) { ctx->err = "unknown iq_format"; return DABB_E_ARG; }
     if (io->iq_is_host || fmt != DABB_IQ_CF32) {
-        const size_t need = (size_t)S * io->buf_len, bps = bytes_per_sample(fmt);
+        const size_t need = (size_t)S * io->buf_len, bps = (size_t)bytes_per_sample(fmt);
         if (fmt == DABB_IQ_CF32) {
             if ((rc = grow(ctx, ctx->d_iq_stage, need))) return rc;
             CK(cudaMemcpy2DAsync(ctx->d_iq_stage, (size_t)io->buf_len * bps, io->iq, (size_t)stride * bps, (size_t)io->buf_len * bps, S, cudaMemcpyHostToDevice, A));
@@ -1082,7 +1073,7 @@ int dabb_submit(dabb_ctx* ctx, const dabb_io* io)
     dabb_ctx::Pending& p = ctx->pend[(ctx->pend_head + ctx->pend_count) & 1];
     if ((rc = prepare_pending(ctx, p))) return rc;
     cudaStream_t A = ctx->stream, Cs = ctx->streamC;
-    const size_t bps = bytes_per_sample(fmt);
+    const size_t bps = (size_t)bytes_per_sample(fmt);
     const size_t need = (size_t)S * io->buf_len * bps;
     if (need > ctx->d_stage2[slot].size()) {
         if ((rc = grow(ctx, ctx->d_stage2[slot], need))) return rc;
@@ -1393,5 +1384,129 @@ int dabb_dev_alloc(dabb_ctx* ctx, size_t bytes, void** out) { if (!ctx || !out) 
 int dabb_dev_free(dabb_ctx* ctx, void* p) { if (!ctx) return DABB_E_ARG; cudaSetDevice(ctx->device); CK(cudaStreamSynchronize(ctx->stream)); CK(cudaFree(p)); return 0; }
 int dabb_memcpy_h2d(dabb_ctx* ctx, void* d, const void* s, size_t n) { if (!ctx) return DABB_E_ARG; cudaSetDevice(ctx->device); CK(cudaMemcpyAsync(d, s, n, cudaMemcpyHostToDevice, ctx->stream)); CK(cudaStreamSynchronize(ctx->stream)); return 0; }
 int dabb_memcpy_d2h(dabb_ctx* ctx, void* d, const void* s, size_t n) { if (!ctx) return DABB_E_ARG; cudaSetDevice(ctx->device); CK(cudaStreamSynchronize(ctx->stream)); CK(cudaMemcpy(d, s, n, cudaMemcpyDeviceToHost)); return 0; }
+
+} // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------
+// wideband channelizer (chan.cu, chan_core.cuh): the filter, the channel table and per-call staging, owned by one context
+
+struct dabb_chan {
+    dabb_ctx* ctx = nullptr;
+    dabb_channel::Geometry g{}; int fmt = 0, n_in = 0, n_ch = 0, block_out = 0; float inv_r = 0.f;
+    std::vector<int32_t> input_of;
+    DevBuf<dabb_channel::f4> d_taps; DevBuf<int32_t> d_input_of; DevBuf<int64_t> d_fmod;
+    DevBuf<int64_t> d_starts;           // per call: out_start [n_ch], then in_start [n_in]
+    DevBuf<uint8_t> d_stage;            // host inputs, copied to the device
+};
+
+namespace {
+constexpr int64_t CHAN_MAX_INDEX = int64_t(1) << 60;      // |in_start| and in_len bounds: index sums stay far from overflow
+
+int chan_range(const dabb_chan* ch, int64_t out_start, int64_t out_len, int64_t& first, int64_t& end)
+{
+    if (out_start < 0 || out_len < 1 || out_len > dabb_channel::MAX_OUT_INDEX || out_start > dabb_channel::MAX_OUT_INDEX - out_len) return DABB_E_ARG;
+    first = dabb_channel::last_input(out_start, ch->g.L, ch->g.M) - ch->g.T + 1;
+    end = dabb_channel::last_input(out_start + out_len - 1, ch->g.L, ch->g.M) + 1;
+    return DABB_OK;
+}
+} // namespace
+
+extern "C" {
+
+int dabb_chan_create(dabb_ctx* ctx, const dabb_chan_config* cfg, dabb_chan** out)
+{
+    if (!ctx || !cfg || !out) return DABB_E_ARG;
+    *out = nullptr;
+    dabb_channel::Geometry g{};
+    if (dabb_channel::geometry(cfg->rate_hz, g) != DABB_OK) {
+        ctx->err = "channelizer: rate " + std::to_string(cfg->rate_hz) + " Hz is outside 2048000 .. 64000000 or 2048000 / rate does not reduce to L / M with L <= 1024";
+        return DABB_E_UNSUPPORTED;
+    }
+    const int nc = cfg->n_channels, ni = cfg->n_inputs;
+    if (cfg->iq_format < DABB_IQ_CF32 || cfg->iq_format > DABB_IQ_S16BE || ni < 1 || ni > dabb_channel::MAX_CHANNELS || nc < 1 || nc > dabb_channel::MAX_CHANNELS
+        || !cfg->input_of_channel || !cfg->offset_hz) { ctx->err = "channelizer: bad format, input count, channel count or NULL channel table"; return DABB_E_ARG; }
+    for (int c = 0; c < nc; c++) {
+        if (cfg->input_of_channel[c] < 0 || cfg->input_of_channel[c] >= ni) { ctx->err = "channelizer: channel " + std::to_string(c) + " names no input"; return DABB_E_ARG; }
+        if (!dabb_channel::offset_ok(g.R, cfg->offset_hz[c])) { ctx->err = "channelizer: offset of channel " + std::to_string(c) + " leaves the input band (|f| + 768000 > R / 2)"; return DABB_E_ARG; }
+    }
+    cudaSetDevice(ctx->device);
+    std::unique_ptr<dabb_chan> ch(new dabb_chan);
+    ch->ctx = ctx; ch->g = g; ch->fmt = cfg->iq_format; ch->n_in = ni; ch->n_ch = nc;
+    ch->block_out = chan_block_outputs(g.L, g.M, g.TP); ch->inv_r = (float)(1.0 / (double)g.R);
+    ch->input_of.assign(cfg->input_of_channel, cfg->input_of_channel + nc);
+    std::vector<float> h((size_t)g.L * g.T), packed((size_t)g.L * g.TP);
+    dabb_channel::design_taps(g, h.data());
+    dabb_channel::pack_taps(g, h.data(), packed.data());
+    std::vector<int64_t> fm((size_t)nc);
+    for (int c = 0; c < nc; c++) fm[(size_t)c] = dabb_channel::floor_mod(cfg->offset_hz[c], g.R);
+    int rc;
+    if ((rc = alloc(ctx, ch->d_taps, packed.size() / 4)) || (rc = alloc(ctx, ch->d_input_of, (size_t)nc)) || (rc = alloc(ctx, ch->d_fmod, (size_t)nc))
+        || (rc = alloc(ctx, ch->d_starts, (size_t)(nc + ni)))) return rc;
+    CK(cudaMemcpy(ch->d_taps, packed.data(), packed.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(ch->d_input_of, ch->input_of.data(), (size_t)nc * sizeof(int32_t), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(ch->d_fmod, fm.data(), (size_t)nc * sizeof(int64_t), cudaMemcpyHostToDevice));
+    *out = ch.release();
+    return DABB_OK;
+}
+
+void dabb_chan_destroy(dabb_chan* ch)
+{
+    if (!ch) return;
+    cudaSetDevice(ch->ctx->device);
+    cudaStreamSynchronize(ch->ctx->stream);
+    delete ch;          // frees its device buffers
+}
+
+int dabb_chan_input_range(const dabb_chan* ch, int64_t out_start, int64_t out_len, int64_t* in_first, int64_t* in_end)
+{
+    if (!ch || !in_first || !in_end) return DABB_E_ARG;
+    int64_t f, e;
+    const int rc = chan_range(ch, out_start, out_len, f, e);
+    if (rc) return rc;
+    *in_first = f; *in_end = e;
+    return DABB_OK;
+}
+
+int dabb_channelize(dabb_chan* ch, const dabb_chan_io* io)
+{
+    if (!ch) return DABB_E_ARG;
+    dabb_ctx* ctx = ch->ctx;
+    if (!io || !io->in || !io->in_start || !io->out || !io->out_start) { ctx->err = "dabb_channelize: NULL argument"; return DABB_E_ARG; }
+    if ((io->in_is_host != 0 && io->in_is_host != 1) || io->in_len < 1 || io->in_len > CHAN_MAX_INDEX || io->in_stride < io->in_len || io->out_len < 1
+        || io->out_stride < io->out_len) { ctx->err = "dabb_channelize: bad in_is_host, length or stride"; return DABB_E_ARG; }
+    for (int i = 0; i < ch->n_in; i++)
+        if (io->in_start[i] < -CHAN_MAX_INDEX || io->in_start[i] > CHAN_MAX_INDEX) { ctx->err = "dabb_channelize: in_start out of range"; return DABB_E_ARG; }
+    for (int c = 0; c < ch->n_ch; c++) {
+        int64_t f, e;
+        const int i = ch->input_of[(size_t)c];
+        if (chan_range(ch, io->out_start[c], io->out_len, f, e) || f < io->in_start[i] || e > io->in_start[i] + io->in_len) {
+            ctx->err = "dabb_channelize: channel " + std::to_string(c) + " needs input samples its buffer does not hold (see dabb_chan_input_range)";
+            return DABB_E_ARG;
+        }
+    }
+    cudaSetDevice(ctx->device);
+    cudaStream_t st = ctx->stream;
+    const size_t bps = (size_t)bytes_per_sample(ch->fmt);
+    std::vector<int64_t> starts((size_t)(ch->n_ch + ch->n_in));
+    std::copy(io->out_start, io->out_start + ch->n_ch, starts.begin());
+    std::copy(io->in_start, io->in_start + ch->n_in, starts.begin() + ch->n_ch);
+    CK(cudaMemcpyAsync(ch->d_starts, starts.data(), starts.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    const uint8_t* in = static_cast<const uint8_t*>(io->in);
+    int64_t in_stride = io->in_stride;
+    if (io->in_is_host) {
+        int rc;
+        if ((rc = grow(ctx, ch->d_stage, (size_t)ch->n_in * (size_t)io->in_len * bps))) return rc;
+        CK(cudaMemcpy2DAsync(ch->d_stage, (size_t)io->in_len * bps, io->in, (size_t)io->in_stride * bps, (size_t)io->in_len * bps, (size_t)ch->n_in, cudaMemcpyHostToDevice, st));
+        in = ch->d_stage; in_stride = io->in_len;
+    }
+    prof_mark(ctx, "__step_begin");
+    ChanParams p{};
+    p.in = in; p.in_stride = in_stride; p.fmt = ch->fmt; p.in_start = ch->d_starts + ch->n_ch; p.in_len = io->in_len;
+    p.input_of = ch->d_input_of; p.fmod = ch->d_fmod; p.out_start = ch->d_starts;
+    p.out_len = io->out_len; p.out = reinterpret_cast<float2*>(io->out); p.out_stride = io->out_stride;
+    p.taps = ch->d_taps; p.R = ch->g.R; p.L = ch->g.L; p.M = ch->g.M; p.T = ch->g.T; p.TP = ch->g.TP; p.inv_r = ch->inv_r; p.block_out = ch->block_out;
+    CK(launch_chan(p, ch->n_ch, st));
+    return check_launch(ctx, "chan_kernel");
+}
 
 } // extern "C"

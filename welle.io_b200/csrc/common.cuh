@@ -6,6 +6,7 @@
 #include "ofdm_core.cuh"
 #include "tii_core.cuh"
 #include "ber_core.cuh"
+#include "chan_core.cuh"
 
 namespace dabb {
 
@@ -95,6 +96,25 @@ struct TiiParams {
 };
 void launch_tii_plan(const TiiParams& p, cudaStream_t st);
 void launch_tii_phase(const TiiParams& p, cudaStream_t st);
+
+// ---- wideband channelizer (chan.cu, chan_core.cuh) ----
+constexpr int CHAN_THREADS = 256;
+struct ChanParams {
+    const uint8_t* in; int64_t in_stride; int fmt; // input i at in + i * in_stride samples of format fmt (DABB_IQ_*)
+    const int64_t* in_start; int64_t in_len;     // [n_inputs] absolute index of each buffer's first sample; samples per buffer
+    const int32_t* input_of;                     // [n_channels] input of each channel
+    const int64_t* fmod;                         // [n_channels] offset_hz mod R
+    const int64_t* out_start;                    // [n_channels] absolute output index of each row's first sample
+    int64_t out_len; float2* out; int64_t out_stride;
+    const dabb_channel::f4* taps;                   // [TP / 4][L] (dabb_channel::pack_taps)
+    int64_t R; int L, M, T, TP; float inv_r;     // inv_r = 1 / R rounded to float
+    int block_out;                               // outputs per CTA (chan_block_outputs)
+};
+// outputs per CTA: 4, 2 or 1 per thread, the most whose input span fits 64 KB of shared memory
+int chan_block_outputs(int L, int M, int TP);
+// input samples a CTA of block_out outputs stages, at most
+int64_t chan_span_cap(int block_out, int L, int M, int TP);
+cudaError_t launch_chan(const ChanParams& p, int n_channels, cudaStream_t st);
 
 // ---- host-side table builders (tables.cpp) ----
 struct HostTables {

@@ -6,6 +6,8 @@ is present, construction fails loudly.
 import ctypes as C
 import os
 import subprocess
+import weakref
+
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -81,7 +83,18 @@ class IO(C.Structure):
 EXPORTS = ["dabb_create", "dabb_destroy", "dabb_last_error", "dabb_abi_version", "dabb_stream_reset", "dabb_set_options", "dabb_get_info", "dabb_select_subchannel",
            "dabb_remove_subchannel", "dabb_process", "dabb_process_async", "dabb_sync", "dabb_join_lanes", "dabb_submit", "dabb_collect", "dabb_cuda_stream", "dabb_kernel_launches",
            "dabb_read_tap", "dabb_profile", "dabb_profile_read", "dabb_ofdm_demod", "dabb_find_index", "dabb_find_index_ex", "dabb_coarse_estimate", "dabb_viterbi", "dabb_fic_decode", "dabb_msc_decode",
-           "dabb_rs_superframes", "dabb_dev_alloc", "dabb_dev_free", "dabb_memcpy_h2d", "dabb_memcpy_d2h"]
+           "dabb_rs_superframes", "dabb_dev_alloc", "dabb_dev_free", "dabb_memcpy_h2d", "dabb_memcpy_d2h",
+           "dabb_chan_create", "dabb_chan_destroy", "dabb_chan_input_range", "dabb_channelize"]
+
+
+class ChanConfig(C.Structure):
+    _fields_ = [("rate_hz", C.c_int64), ("iq_format", C.c_int32), ("n_inputs", C.c_int32), ("n_channels", C.c_int32), ("reserved", C.c_int32),
+                ("input_of_channel", C.c_void_p), ("offset_hz", C.c_void_p)]
+
+
+class ChanIO(C.Structure):
+    _fields_ = [("in_", C.c_void_p), ("in_is_host", C.c_int32), ("in_stride", C.c_int64), ("in_start", C.c_void_p), ("in_len", C.c_int64),
+                ("out", C.c_void_p), ("out_stride", C.c_int64), ("out_start", C.c_void_p), ("out_len", C.c_int64)]
 
 
 def build():
@@ -101,6 +114,8 @@ def load_library():
     lib.dabb_kernel_launches.argtypes = [C.c_void_p]
     lib.dabb_destroy.argtypes = [C.c_void_p]
     lib.dabb_destroy.restype = None
+    lib.dabb_chan_destroy.argtypes = [C.c_void_p]
+    lib.dabb_chan_destroy.restype = None
     return lib
 
 
@@ -174,6 +189,7 @@ class Context:
             raise DabbError(f"dabb_create failed ({rc}): {self.lib.dabb_last_error(None).decode()}")
         self.h, self.n_streams, self.n_slots = h, n_streams, max(1, n_subch_slots)
         self._bufs = []
+        self._chans = weakref.WeakSet()         # channelizers of this context: close() destroys them before the context
 
     def _ck(self, rc):
         if rc != 0:
@@ -181,6 +197,8 @@ class Context:
 
     def close(self):
         if getattr(self, "h", None):
+            for ch in list(getattr(self, "_chans", ())):
+                ch.destroy()
             self.lib.dabb_destroy(self.h)
             self.h = None
 
@@ -426,3 +444,63 @@ class Context:
         out = d_s.download(np.uint8).reshape(n, sf_len); info = d_i.download(np.int32).reshape(n, 4)
         d_s.free(); d_i.free()
         return out, info
+
+
+class Channelizer:
+    """Wideband channelizer of a context (dabb_chan_create): `offsets_hz[c]` is the centre of channel c in input
+    `input_of_channel[c]` (default: all channels read input 0), every input at `rate_hz` in `iq_format` (IQ_*); `n_inputs` defaults to
+    one more than the largest input a channel reads.  run() turns the inputs' samples into each channel's 2.048 Msps samples [out_start[c], out_start[c] + out_len) on the device, in a buffer that
+    Context.process takes as its iq (stride = out_stride, buf_start = out_start).  Stateless: any range can be asked for at any time.
+    destroy() (or the object's end) frees it and is safe to call twice; Context.close destroys the context's remaining channelizers
+    first, so a channelizer never outlives its context."""
+
+    def __init__(self, ctx, rate_hz, offsets_hz, input_of_channel=None, iq_format=IQ_CF32, n_inputs=None):
+        self.ctx, self.lib = ctx, ctx.lib
+        self.offsets = np.ascontiguousarray(offsets_hz, np.int64).reshape(-1)
+        n = self.offsets.size
+        self.input_of = np.ascontiguousarray(np.zeros(n, np.int32) if input_of_channel is None else input_of_channel, np.int32).reshape(-1)
+        self.n_channels = n
+        self.n_inputs = int(self.input_of.max()) + 1 if n_inputs is None and n else int(n_inputs or 1)
+        self.rate_hz, self.iq_format = int(rate_hz), int(iq_format)
+        cfg = ChanConfig(self.rate_hz, self.iq_format, self.n_inputs, n, 0, self.input_of.ctypes.data, self.offsets.ctypes.data)
+        h = C.c_void_p()
+        ctx._ck(self.lib.dabb_chan_create(ctx.h, C.byref(cfg), C.byref(h)))
+        self.h = h
+        ctx._chans.add(self)
+
+    def input_range(self, out_start, out_len):
+        """[first, end): the absolute input samples that outputs [out_start, out_start + out_len) of any channel read"""
+        f, e = C.c_int64(), C.c_int64()
+        self.ctx._ck(self.lib.dabb_chan_input_range(self.h, C.c_int64(int(out_start)), C.c_int64(int(out_len)), C.byref(f), C.byref(e)))
+        return f.value, e.value
+
+    def run(self, x, in_start, in_len, out_start, out_len, in_stride=None, in_is_host=None, out=None, out_stride=None):
+        """x: the inputs, [n_inputs, in_stride] samples (numpy: host, copied in the call; DevBuf / int address: device) whose first
+        samples are the absolute indices in_start[i].  out_start: one absolute output index per channel (an int: the same for all).
+        Returns the device buffer (float2 [n_channels][out_stride]); `out` reuses one."""
+        if in_is_host is None:
+            in_is_host = isinstance(x, np.ndarray)
+        if in_stride is None:           # a numpy array [n_inputs, ...]: one row per input
+            in_stride = x.reshape(self.n_inputs, -1)[0].nbytes // (8, 2, 2, 4, 4)[self.iq_format]
+        ins = np.ascontiguousarray(np.broadcast_to(np.asarray(in_start, np.int64), (self.n_inputs,)))
+        outs = np.ascontiguousarray(np.broadcast_to(np.asarray(out_start, np.int64), (self.n_channels,)))
+        out_stride = int(out_len if out_stride is None else out_stride)
+        if out is None:
+            out = self.ctx.dev(self.n_channels * out_stride * 8)
+        xa = np.ascontiguousarray(x) if isinstance(x, np.ndarray) else None
+        io = ChanIO(_addr(xa if xa is not None else x), int(bool(in_is_host)), int(in_stride), ins.ctypes.data, int(in_len),
+                    _addr(out), out_stride, outs.ctypes.data, int(out_len))
+        self.ctx._ck(self.lib.dabb_channelize(self.h, C.byref(io)))
+        return out
+
+    def destroy(self):
+        if getattr(self, "h", None):
+            self.lib.dabb_chan_destroy(self.h)
+            self.ctx._chans.discard(self)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
