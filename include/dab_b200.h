@@ -313,6 +313,48 @@ typedef struct {
 int dabb_channelize(dabb_chan* ch, const dabb_chan_io* io);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Spectrum survey: where the ensembles of a wideband recording are, before anything is decoded.
+ * replaces: the reference's channel scan (CRadioController::startScan / nextChannel, welle-gui/radio_controller.cpp:406,902), which
+ * retunes the receiver channel by channel and waits for onSignalPresence; a recording cannot be retuned, so the whole band is looked at
+ * at once and each candidate is then confirmed by decoding it (batch_decode --scan).
+ *
+ * dabb_survey: the averaged power spectrum of each of n_inputs inputs of in_len samples (input i at in + i * in_stride samples, in
+ * iq_format, converted exactly like dabb_channelize / CRAWFile::convertSamples; host with in_is_host = 1, else device).  Welch segments
+ * of nfft samples (a power of two, 1024 .. 16384) with 50 % overlap: S = floor((in_len - nfft) / (nfft/2)) + 1 segments, segment s
+ * starting at sample s * nfft/2 (samples past the last segment are not read).  With the periodic Hann window w[n] = sin^2(pi n / nfft):
+ *     P[j] = (1/S) sum_s |sum_n w[n] x[s nfft/2 + n] exp(-2 pi i k n / nfft)|^2 / sum_n w[n]^2,   k = (j + nfft/2) mod nfft
+ * so bin j is at frequency (j - nfft/2) R / nfft, from -R/2 up to R/2 (R the input's sample rate; the survey does not need it).
+ * psd is HOST float [n_inputs][nfft], written when the call returns.  The transform is fp32 (every P[j] within 1e-4 P[j] + 1e-7 mean(P)
+ * of the exact value in the tests); the segments are summed in a fixed order without atomics, so the same call gives the same bits.
+ * The work runs on the context's main stream; scratch is allocated on the first call and kept until dabb_destroy (a context that never
+ * surveys allocates nothing).  Arguments are checked before anything is enqueued: a NULL pointer, a bad nfft, format or in_is_host,
+ * n_inputs outside 1 .. 4096, in_len < nfft or in_stride < in_len returns DABB_E_ARG and writes nothing. */
+typedef struct {
+    const void* in; int32_t in_is_host; int32_t iq_format;
+    int64_t in_stride; int32_t n_inputs; int32_t nfft;
+    int64_t in_len;
+    float* psd;
+} dabb_survey_io;
+int dabb_survey(dabb_ctx* ctx, const dabb_survey_io* io);
+
+/* dabb_survey_candidates: the ensemble candidates of one spectrum psd[nfft] of an input at rate_hz (host code, no context).  With
+ * f_j = (j - nfft/2) R / nfft and L_j = 10 log10(max(P_j, 1e-12 max P)) (no candidates when max P = 0):
+ *   - a centre bin c is considered when |f_c| + 768 000 <= R/2 (the channelizer's rule);
+ *   - its in-band set is I = {j : |f_j - f_c| <= 700 000};
+ *   - its guard sides are G- = {j : 784 000 <= f_c - f_j <= 896 000} and G+ = {j : 784 000 <= f_j - f_c <= 896 000}, each clipped to
+ *     |f_j| <= R/2 - R/nfft; a side is present when it keeps at least ceil(56 000 nfft / R) bins, and c is skipped when neither is
+ *     (the guards lie inside the 176 kHz gap to a neighbour on the 1.712 MHz raster, clear of its 944 kHz edge);
+ *   - score(c) = mean over I of L - the larger mean over the present guard sides (double sums in ascending j), so a centre at the edge
+ *     of a wider signal, with one side inside it, scores about 0 dB;
+ *   - every maximal run of consecutive considered bins with score >= min_score_db is one candidate: offset_hz is the run's midpoint
+ *     ((c_first + c_last - nfft) R) / (2 nfft) rounded to the nearest Hz (ties away from zero), score_db the run's largest score.
+ * Membership is decided by exact integer comparisons.  Candidates are written in ascending offset, at most cap of them; *n_found is
+ * the full count.  DABB_E_ARG for a NULL pointer, a bad nfft, a rate outside 1 .. 64 000 000 or cap < 0. */
+typedef struct { int64_t offset_hz; float score_db; int32_t reserved; } dabb_survey_candidate;
+int dabb_survey_candidates(const float* psd, int32_t nfft, int64_t rate_hz, float min_score_db,
+                           dabb_survey_candidate* out, int32_t cap, int32_t* n_found);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Stage-level entry points (stateless).  Pointers are DEVICE pointers unless named host_*.
  * ------------------------------------------------------------------------------------------------------- */
 

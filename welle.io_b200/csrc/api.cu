@@ -4,6 +4,7 @@
 #include "../../include/dab_b200.h"
 #include "common.cuh"
 #include "viterbi.cuh"
+#include "survey_core.cuh"
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -147,6 +148,8 @@ struct dabb_ctx {
     // optional per-kernel timing: one event after every launch, durations = differences of consecutive events
     bool prof = false; std::vector<cudaEvent_t> prof_ev; std::vector<const char*> prof_name; size_t prof_used = 0;
     std::vector<std::pair<std::string, std::pair<double, long>>> prof_acc;
+    // spectrum survey (survey.cu), allocated by the first dabb_survey: twiddle and window tables, host input staging, per-chunk sums, spectra
+    DevBuf<dabb_channel::cf> d_svy_tw; DevBuf<float> d_svy_win; DevBuf<uint8_t> d_svy_stage; DevBuf<float> d_svy_part, d_svy_psd;
 };
 
 namespace {
@@ -1507,6 +1510,65 @@ int dabb_channelize(dabb_chan* ch, const dabb_chan_io* io)
     p.taps = ch->d_taps; p.R = ch->g.R; p.L = ch->g.L; p.M = ch->g.M; p.T = ch->g.T; p.TP = ch->g.TP; p.inv_r = ch->inv_r; p.block_out = ch->block_out;
     CK(launch_chan(p, ch->n_ch, st));
     return check_launch(ctx, "chan_kernel");
+}
+
+} // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------
+// spectrum survey (survey.cu, survey_core.cuh) and the candidate detector
+
+extern "C" {
+
+int dabb_survey(dabb_ctx* ctx, const dabb_survey_io* io)
+{
+    if (!ctx) return DABB_E_ARG;
+    if (!io || !io->in || !io->psd) { ctx->err = "dabb_survey: NULL argument"; return DABB_E_ARG; }
+    const int log2n = dabb_spectrum::log2_nfft(io->nfft);
+    if (log2n < 0) { ctx->err = "dabb_survey: nfft must be a power of two from 1024 to 16384"; return DABB_E_ARG; }
+    if ((io->in_is_host != 0 && io->in_is_host != 1) || io->iq_format < DABB_IQ_CF32 || io->iq_format > DABB_IQ_S16BE || io->n_inputs < 1
+        || io->n_inputs > dabb_spectrum::MAX_INPUTS || io->in_len < io->nfft || io->in_len > dabb_spectrum::MAX_LEN || io->in_stride < io->in_len) {
+        ctx->err = "dabb_survey: bad in_is_host, format, input count, length or stride"; return DABB_E_ARG;
+    }
+    cudaSetDevice(ctx->device);
+    cudaStream_t st = ctx->stream;
+    int rc;
+    if (!ctx->d_svy_tw) {
+        std::vector<dabb_channel::cf> tw(dabb_spectrum::MAX_NFFT / 2); std::vector<float> win(dabb_spectrum::MAX_NFFT);
+        dabb_spectrum::make_tables(tw.data(), win.data());
+        if ((rc = alloc(ctx, ctx->d_svy_win, win.size())) || (rc = alloc(ctx, ctx->d_svy_tw, tw.size()))) { ctx->d_svy_tw.reset(); return rc; }
+        // pageable sources: each copy has read its source when it returns.  d_svy_tw is what marks the tables as present, so a failed
+        // copy leaves none
+        cudaError_t e = cudaMemcpyAsync(ctx->d_svy_win, win.data(), win.size() * sizeof(float), cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->d_svy_tw, tw.data(), tw.size() * sizeof(dabb_channel::cf), cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) { ctx->d_svy_tw.reset(); ctx->d_svy_win.reset(); ctx->err = std::string("dabb_survey: table upload: ") + cudaGetErrorString(e); return DABB_E_CUDA; }
+    }
+    const int n_in = io->n_inputs, nfft = io->nfft;
+    const size_t bps = (size_t)bytes_per_sample(io->iq_format);
+    const int64_t S = dabb_spectrum::n_segments(io->in_len, nfft), chunk = dabb_spectrum::chunk_segments(S, n_in), n_chunks = (S + chunk - 1) / chunk;
+    const int64_t used = (S + 1) * (nfft / 2);          // the samples the segments read
+    const uint8_t* in = static_cast<const uint8_t*>(io->in);
+    int64_t in_stride = io->in_stride;
+    if (io->in_is_host) {
+        if ((rc = grow(ctx, ctx->d_svy_stage, (size_t)n_in * (size_t)used * bps))) return rc;
+        CK(cudaMemcpy2DAsync(ctx->d_svy_stage, (size_t)used * bps, io->in, (size_t)io->in_stride * bps, (size_t)used * bps, (size_t)n_in, cudaMemcpyHostToDevice, st));
+        in = ctx->d_svy_stage; in_stride = used;
+    }
+    if ((rc = grow(ctx, ctx->d_svy_part, (size_t)n_in * (size_t)n_chunks * (size_t)nfft)) || (rc = grow(ctx, ctx->d_svy_psd, (size_t)n_in * (size_t)nfft))) return rc;
+    prof_mark(ctx, "__step_begin");
+    SurveyParams p{};
+    p.in = in; p.in_stride = in_stride; p.fmt = io->iq_format; p.S = S; p.chunk = chunk; p.tw = ctx->d_svy_tw; p.win = ctx->d_svy_win; p.part = ctx->d_svy_part;
+    CK(launch_survey(p, log2n, n_chunks, n_in, st));
+    if ((rc = check_launch(ctx, "survey_kernel"))) return rc;
+    launch_survey_sum(ctx->d_svy_part, n_chunks, log2n, n_in, 1.0 / ((double)S * (3.0 * nfft / 8.0)), ctx->d_svy_psd, st);
+    if ((rc = check_launch(ctx, "survey_sum_kernel"))) return rc;
+    CK(cudaMemcpyAsync(io->psd, ctx->d_svy_psd, (size_t)n_in * (size_t)nfft * sizeof(float), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return DABB_OK;
+}
+
+int dabb_survey_candidates(const float* psd, int32_t nfft, int64_t rate_hz, float min_score_db, dabb_survey_candidate* out, int32_t cap, int32_t* n_found)
+{
+    return dabb_spectrum::candidates(psd, nfft, rate_hz, min_score_db, out, cap, n_found);
 }
 
 } // extern "C"

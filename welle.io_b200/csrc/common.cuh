@@ -116,6 +116,18 @@ int chan_block_outputs(int L, int M, int TP);
 int64_t chan_span_cap(int block_out, int L, int M, int TP);
 cudaError_t launch_chan(const ChanParams& p, int n_channels, cudaStream_t st);
 
+// ---- spectrum survey (survey.cu, survey_core.cuh) ----
+constexpr int SURVEY_THREADS = 512;
+struct SurveyParams {
+    const uint8_t* in; int64_t in_stride; int fmt;  // input i at in + i * in_stride samples of format fmt (DABB_IQ_*)
+    int64_t S, chunk;                            // segments per input, segments per CTA (the last CTA of an input may have fewer)
+    const dabb_channel::cf* tw; const float* win;   // dabb_spectrum::make_tables
+    float* part;                                 // [n_inputs][n_chunks][nfft] per-chunk sums, storage order
+};
+cudaError_t launch_survey(const SurveyParams& p, int log2n, int64_t n_chunks, int n_inputs, cudaStream_t st);
+// psd[i][j] = scale * sum over the chunks of input i of part at bin j (double, ascending chunk order)
+void launch_survey_sum(const float* part, int64_t n_chunks, int log2n, int n_inputs, double scale, float* psd, cudaStream_t st);
+
 // ---- host-side table builders (tables.cpp) ----
 struct HostTables {
     float2 tw_fwd[TwLayout::TOTAL], tw_inv[TwLayout::TOTAL];

@@ -84,7 +84,7 @@ EXPORTS = ["dabb_create", "dabb_destroy", "dabb_last_error", "dabb_abi_version",
            "dabb_remove_subchannel", "dabb_process", "dabb_process_async", "dabb_sync", "dabb_join_lanes", "dabb_submit", "dabb_collect", "dabb_cuda_stream", "dabb_kernel_launches",
            "dabb_read_tap", "dabb_profile", "dabb_profile_read", "dabb_ofdm_demod", "dabb_find_index", "dabb_find_index_ex", "dabb_coarse_estimate", "dabb_viterbi", "dabb_fic_decode", "dabb_msc_decode",
            "dabb_rs_superframes", "dabb_dev_alloc", "dabb_dev_free", "dabb_memcpy_h2d", "dabb_memcpy_d2h",
-           "dabb_chan_create", "dabb_chan_destroy", "dabb_chan_input_range", "dabb_channelize"]
+           "dabb_chan_create", "dabb_chan_destroy", "dabb_chan_input_range", "dabb_channelize", "dabb_survey", "dabb_survey_candidates"]
 
 
 class ChanConfig(C.Structure):
@@ -95,6 +95,30 @@ class ChanConfig(C.Structure):
 class ChanIO(C.Structure):
     _fields_ = [("in_", C.c_void_p), ("in_is_host", C.c_int32), ("in_stride", C.c_int64), ("in_start", C.c_void_p), ("in_len", C.c_int64),
                 ("out", C.c_void_p), ("out_stride", C.c_int64), ("out_start", C.c_void_p), ("out_len", C.c_int64)]
+
+
+class SurveyIO(C.Structure):
+    _fields_ = [("in_", C.c_void_p), ("in_is_host", C.c_int32), ("iq_format", C.c_int32), ("in_stride", C.c_int64), ("n_inputs", C.c_int32),
+                ("nfft", C.c_int32), ("in_len", C.c_int64), ("psd", C.c_void_p)]
+
+
+# dabb_survey_candidate: one ensemble candidate of a spectrum
+CANDIDATE_DTYPE = np.dtype([("offset_hz", "<i8"), ("score_db", "<f4"), ("reserved", "<i4")])
+
+
+def survey_candidates(psd, rate_hz, min_score_db=6.0):
+    """the ensemble candidates of one spectrum psd[nfft] (Context.survey) of an input at rate_hz (dabb_survey_candidates): a
+    CANDIDATE_DTYPE array in ascending offset_hz"""
+    lib = load_library()
+    p = np.ascontiguousarray(psd, np.float32).reshape(-1)
+    n = C.c_int32()
+    cap = p.size // 2 + 1                       # runs of consecutive bins: never more than every other bin
+    out = np.zeros(cap, CANDIDATE_DTYPE)
+    rc = lib.dabb_survey_candidates(p.ctypes.data_as(C.c_void_p), C.c_int32(p.size), C.c_int64(int(rate_hz)), C.c_float(min_score_db),
+                                    out.ctypes.data_as(C.c_void_p), C.c_int32(cap), C.byref(n))
+    if rc != 0:
+        raise DabbError(f"dabb_survey_candidates failed ({rc}): bad nfft ({p.size}) or rate ({rate_hz})")
+    return out[:n.value]
 
 
 def build():
@@ -360,6 +384,27 @@ class Context:
             out = np.zeros((self.n_streams, TU), np.float32)
         self._ck(self.lib.dabb_read_tap(self.h, what, _vp(out), C.c_size_t(out.nbytes)))
         return out
+
+    def survey(self, x, nfft, in_len=None, iq_format=IQ_CF32, in_is_host=None):
+        """the averaged power spectrum of every input (dabb_survey): a float32 array [n_inputs, nfft] whose bin j is at (j - nfft/2) R / nfft.
+        x: a numpy array [n_inputs, samples] (or one input as a 1-d array; host, copied in the call; raw formats as bytes), or a
+        DevBuf / device address of one input of in_len samples (in_is_host=False)"""
+        if in_is_host is None:
+            in_is_host = isinstance(x, np.ndarray)
+        bps = (8, 2, 2, 4, 4)[iq_format] if 0 <= iq_format <= 4 else 1
+        if isinstance(x, np.ndarray):
+            xa = np.ascontiguousarray(x)
+            rows = xa.reshape(1, -1) if xa.ndim == 1 else xa.reshape(xa.shape[0], -1)
+            n_inputs, stride = rows.shape[0], rows[0].nbytes // bps
+        else:
+            if in_len is None:
+                raise ValueError("Context.survey: device input needs in_len (its length in samples)")
+            xa, n_inputs, stride = x, 1, int(in_len)
+        in_len = stride if in_len is None else int(in_len)
+        psd = np.zeros((n_inputs, int(nfft)), np.float32)
+        io = SurveyIO(_addr(xa), int(bool(in_is_host)), int(iq_format), int(stride), n_inputs, int(nfft), in_len, psd.ctypes.data)
+        self._ck(self.lib.dabb_survey(self.h, C.byref(io)))
+        return psd
 
     # ---- stage-level (numpy in / numpy out; device staging through the ABI)
     def ofdm_demod(self, iq_frames, prs_start, nco=None, want_r1=False, want_fc=False):
