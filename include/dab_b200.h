@@ -82,8 +82,27 @@ typedef struct {
     int32_t decode_tii;         /* RadioReceiverOptions::decodeTII: analyse the transmitter identification of every decoded frame on the device
                                    (tap 9); with keep_taps, also produce tap 4 (the two spectra TIIDecoder starts from) */
     int32_t count_bit_errors;   /* count the channel bit errors of the FIC and of every decoded sub-channel codeword on the device (tap 10) */
-    int32_t reserved[3];
+    int32_t soft_demap;         /* DABB_DEMAP_*: how the OFDM demodulator turns each carrier into softbits (see below); a value outside the
+                                   enum is refused with DABB_E_ARG and the call changes nothing */
+    int32_t reserved[2];
 } dabb_options;
+
+/* Soft-decision demap of the OFDM demodulator, dabb_options.soft_demap; takes effect from the next step, and dabb_ofdm_demod uses the
+ * context's current value.
+ * DABB_DEMAP_REFERENCE (0, the default) is OfdmDecoder::decodeDataSymbol (ofdm-decoder.cpp:198-219): for data symbol l and carrier k,
+ *   r1 = X_l[k] conj(X_{l-1}[k]), l1 = |Re r1| + |Im r1|, softbit = trunc(-Re/Im(r1) * 127 / l1)
+ * It divides away every carrier's amplitude, so a carrier in a deep multipath notch is as confident as the strongest one.
+ * DABB_DEMAP_WEIGHTED (replaces: none; it deviates from ofdm-decoder.cpp:208-214) scales weak carriers down:
+ *   G_l = 2^(mean over the symbol's 1536 carriers of log2(max(l1, 2^-126))), the geometric mean of the carrier levels
+ *   softbit = trunc(-Re/Im(r1) * 127 / max(l1, G_l))
+ * A carrier with l1 >= G_l gets exactly the reference softbits; a weaker one gets them scaled by l1 / G_l, never more confidence than
+ * the reference gives it; |softbit| <= 127.  The geometric mean is barely moved by a few very strong carriers (a narrowband interferer),
+ * unlike the arithmetic mean.  G_l = 0 (the reference demap for the whole symbol) when any l1 of the symbol is inf or NaN.  G_l is
+ * within 1e-5 relative of its float64 value and is computed inside the CTA that transforms the symbol in a fixed order, so the softbits
+ * do not depend on the batch size or the launch configuration.  r1_out (tap 2's constellation, dabb_ofdm_demod's r1_out) is the same in
+ * both modes.  The FIC, MSC, BER and TII paths read the softbits unchanged; more softbits truncate to 0, so tap 10 counts more
+ * erasures. */
+enum { DABB_DEMAP_REFERENCE = 0, DABB_DEMAP_WEIGHTED = 1 };
 
 /* Channel bit errors of one stream in one step: tap 10, while dabb_options.count_bit_errors is set.  Per codeword (a FIC block of 768
  * bits, or a logical frame of 24 * bitrate bits) the decoded bits before energy dispersal (the output bytes MSB first, XOR the PRBS; 6
@@ -362,7 +381,8 @@ int dabb_survey_candidates(const float* psd, int32_t nfft, int64_t rate_hz, floa
  * Frame f: PRS useful part at iq + f*stride + prs_start[f] (2048 samples) followed by 75 symbols of 2552 samples.
  * soft_out: int8 [n][75][3072]; r1_out (may be NULL): float2 [n][75][1536] pre-quantisation products;
  * freqcorr_out (may be NULL): float2 [n] CP correlation sums (ofdm-processor.cpp:436-442).
- * nco (may be NULL): int32 [n][2] = {localPhase at the first PRS sample, phase increment Hz} (ofdm-processor.cpp:211-214) */
+ * nco (may be NULL): int32 [n][2] = {localPhase at the first PRS sample, phase increment Hz} (ofdm-processor.cpp:211-214).
+ * The softbits follow the context's dabb_options.soft_demap (DABB_DEMAP_*); r1_out does not depend on it. */
 int dabb_ofdm_demod(dabb_ctx* ctx, const float* iq, int64_t stride_samples, const int64_t* prs_start, int32_t n_frames,
                     const int32_t* nco, int8_t* soft_out, float* r1_out, float* freqcorr_out);
 

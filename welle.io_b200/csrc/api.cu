@@ -143,7 +143,7 @@ struct dabb_ctx {
         std::vector<int32_t> flen;      // [slot][stream] the stream's logical frame length when the step was enqueued (0: nothing to deliver)
     } pend[2], pend_sync;     // the two dabb_submit slots; dabb_process and taps 7 / 8, which never leave a step outstanding
     int pend_head = 0, pend_count = 0; int64_t submits = 0;
-    int groups = 1; int fc_pitch = 1; int tail_frames = 0; int nco_fast = 0;
+    int groups = 1; int fc_pitch = 1; int tail_frames = 0; int nco_fast = 0; int soft_demap = DABB_DEMAP_REFERENCE;
     DevBuf<const int32_t*> d_info_tab;
     // optional per-kernel timing: one event after every launch, durations = differences of consecutive events
     bool prof = false; std::vector<cudaEvent_t> prof_ev; std::vector<const char*> prof_name; size_t prof_used = 0;
@@ -965,7 +965,7 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     OfdmParams op{}; op.iq = iq; op.stride = stride; op.prs_start = d_prs; op.nco = d_nco_frame; op.active = d_active; op.soft = d_soft; op.soft_stride = DABB_SOFT_PER_FRAME;
     op.r1 = ctx->d_r1; op.freqcorr = d_fc; op.level = d_lvl; op.snr = d_snr; op.n_frames = S; op.groups = ctx->groups; op.sym_per_cta = 75 / ctx->groups;
     op.trace = ctx->trace;
-    op.n_full = S - ctx->tail_frames; op.tail_groups = ctx->tail_frames ? OFDM_TAIL_GROUPS : 1; op.fc_pitch = ctx->fc_pitch; op.nco_fast = ctx->nco_fast;
+    op.n_full = S - ctx->tail_frames; op.tail_groups = ctx->tail_frames ? OFDM_TAIL_GROUPS : 1; op.fc_pitch = ctx->fc_pitch; op.nco_fast = ctx->nco_fast; op.weighted = ctx->soft_demap == DABB_DEMAP_WEIGHTED;
     launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, A);
     if ((rc = check_launch(ctx, "ofdm_demod_kernel"))) return rc;
     advance_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, S, ctx->fc_pitch, d_fc, d_lvl);
@@ -1197,7 +1197,7 @@ int dabb_ofdm_demod(dabb_ctx* ctx, const float* iq, int64_t stride, const int64_
     sync_all(ctx);
     OfdmParams op{}; op.iq = reinterpret_cast<const float2*>(iq); op.stride = stride; op.prs_start = prs_start; op.active = nullptr; op.soft = soft; op.soft_stride = DABB_SOFT_PER_FRAME;
     op.r1 = reinterpret_cast<float2*>(r1); op.freqcorr = reinterpret_cast<float2*>(fc); op.snr = nullptr; op.n_frames = n;
-    op.groups = (fc || n >= 1024) ? 1 : (n >= 64 ? 5 : 25); op.sym_per_cta = 75 / op.groups; op.n_full = n; op.tail_groups = 1; op.fc_pitch = op.groups; op.nco_fast = ctx->nco_fast;
+    op.groups = (fc || n >= 1024) ? 1 : (n >= 64 ? 5 : 25); op.sym_per_cta = 75 / op.groups; op.n_full = n; op.tail_groups = 1; op.fc_pitch = op.groups; op.nco_fast = ctx->nco_fast; op.weighted = ctx->soft_demap == DABB_DEMAP_WEIGHTED;
     DevBuf<int32_t> nco4;
     int rc;
     if (nco) {
@@ -1259,7 +1259,8 @@ int dabb_get_info(dabb_ctx* ctx, int32_t what, int64_t* out)
 
 int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
 {
-    if (!ctx || !opt || opt->fft_placement < 0 || opt->fft_placement > 2 || opt->freqsync_method < 0 || opt->freqsync_method > 2) return DABB_E_ARG;
+    if (!ctx || !opt || opt->fft_placement < 0 || opt->fft_placement > 2 || opt->freqsync_method < 0 || opt->freqsync_method > 2
+        || (opt->soft_demap != DABB_DEMAP_REFERENCE && opt->soft_demap != DABB_DEMAP_WEIGHTED)) return DABB_E_ARG;
     if (opt->decode_tii && !ctx->d_tii_res) {       // first use of TII: its buffers (64 KB per stream), zeroed = no open combinations
         cudaSetDevice(ctx->device);
         sync_all(ctx);
@@ -1287,7 +1288,7 @@ int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
         CK(cudaStreamSynchronize(ctx->stream));
     }
     ctx->disable_coarse = opt->disable_coarse != 0; ctx->placement = opt->fft_placement; ctx->freqsync = opt->freqsync_method; ctx->decode_tii = opt->decode_tii != 0;
-    ctx->count_ber = opt->count_bit_errors != 0;
+    ctx->count_ber = opt->count_bit_errors != 0; ctx->soft_demap = opt->soft_demap;
     return DABB_OK;
 }
 

@@ -57,6 +57,7 @@ struct OfdmParams {
     int n_full; int tail_groups;                 // frames >= n_full are cut into tail_groups CTAs each (tail_groups divides 75; 1 / 0 = off)
     int fc_pitch;                                // freqcorr entries per frame (>= groups, tail_groups); 0 -> the larger of the two
     int nco_fast;                                // DABB_NCO_FAST: fp32 oscillator (tolerance mode)
+    int weighted;                                // DABB_DEMAP_WEIGHTED: softbits against max(carrier level, the symbol's geometric-mean level)
     TraceBuf trace;                              // rec == nullptr: off
 };
 

@@ -101,6 +101,20 @@ __device__ __forceinline__ float block_sum(float v, float* red, int t)
     return red[0] + red[1] + red[2] + red[3];
 }
 
+// the CTA's sum of the per-thread level sums (DABB_DEMAP_WEIGHTED) in the fixed order of block_sum
+__device__ __forceinline__ LevelSum block_level_sum(LevelSum a, float* red, int t)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { a.e += __shfl_down_sync(0xffffffffu, a.e, o); a.m += __shfl_down_sync(0xffffffffu, a.m, o); }
+    __syncthreads();
+    if ((t & 31) == 0) { red[t >> 5] = a.m; red[4 + (t >> 5)] = __int_as_float(a.e); }
+    __syncthreads();
+    LevelSum r;
+    r.m = red[0] + red[1] + red[2] + red[3];
+    r.e = __float_as_int(red[4]) + __float_as_int(red[5]) + __float_as_int(red[6]) + __float_as_int(red[7]);
+    return r;
+}
+
 // per-thread loop-invariant shared-memory indices of the exchange buffer (see swz() in ofdm_core.cuh)
 struct XIdx {
     int a[2];     // pass A: swz(8 * rev(n0)) for the two blocks; element e lives at a[h] ^ e
@@ -319,7 +333,7 @@ __device__ __forceinline__ void fft2048_finish(float2 v[16], DemodSmem& sm, int 
 #endif
 }
 
-template <bool EXACT, bool TAP, bool FASTNCO>
+template <bool EXACT, bool TAP, bool FASTNCO, bool WEIGHTED>
 __global__ void __launch_bounds__(OFDM_THREADS, DEMOD_CTAS_PER_SM)
 ofdm_demod_kernel(DevTables tb, OfdmParams p)
 {
@@ -408,6 +422,28 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
         fft2048_finish<EXACT>(v, sm, t, xi, tw_c5, b2);   // contains barrier (2)
 
         if (l >= l_first) {
+            if (WEIGHTED) {
+                // DABB_DEMAP_WEIGHTED: r1 of every owned bin into v[] (its spectrum moves to prev[]), the symbol's geometric-mean carrier
+                // level G from one block reduction, then the demap against max(l1, G) (ofdm_core.cuh: level_acc, level_gmean)
+                LevelSum ls{0, 0.f};
+#pragma unroll
+                for (int s = 0; s < NSLOT; s++) {
+                    const float2 X = v[slot_c(s)];
+                    v[slot_c(s)] = diff_one<EXACT>(X, prev[s]);
+                    prev[s] = X;
+                    if (sidx[s] < SB_DUMMY) level_acc(ls, level_l1(v[slot_c(s)]));
+                }
+                const LevelSum tot = block_level_sum(ls, sm.red, t);
+                const float G = level_gmean(tot), rG = q127(G);
+#pragma unroll
+                for (int s = 0; s < NSLOT; s++) {
+                    const float2 r1 = v[slot_c(s)];
+                    int8_t sre, sim;
+                    demap_weighted(r1, G, rG, sre, sim);
+                    sbuf[sidx[s]] = (uint16_t)((uint8_t)sre | ((uint16_t)(uint8_t)sim << 8));
+                    if (TAP) { const int c0 = tb.invperm[t + 128 * slot_c(s)]; if (c0 >= 0) p.r1[((int64_t)f * 75 + (l - 1)) * KC + c0] = r1; }
+                }
+            } else {
             // demap owned bins against the previous symbol, scatter softbits into logical order (branch free)
 #pragma unroll
             for (int s = 0; s < NSLOT; s++) {
@@ -417,6 +453,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
                 sbuf[sidx[s]] = (uint16_t)((uint8_t)sre | ((uint16_t)(uint8_t)sim << 8));
                 if (TAP) { const int c0 = tb.invperm[t + 128 * slot_c(s)]; if (c0 >= 0) p.r1[((int64_t)f * 75 + (l - 1)) * KC + c0] = r1; }
                 prev[s] = X;
+            }
             }
             __syncthreads();                   // (3)
             // de-interleave the pairs into the reference's layout (1536 Re bits, then 1536 Im bits): thread t < 96 takes the 16-byte
@@ -970,11 +1007,13 @@ void launch_ofdm_demod(const DevTables& tb, const OfdmParams& p_in, int fft_mode
     const size_t sm = sizeof(DemodSmem);
     const dim3 grid(p.n_full * p.groups + (p.n_frames - p.n_full) * p.tail_groups), block(OFDM_THREADS);
     const bool tap = p.r1 != nullptr, fast = p.nco_fast != 0 && p.nco != nullptr;
-#define LAUNCH(E, T, F) do { set_smem(ofdm_demod_kernel<E, T, F>, sm); ofdm_demod_kernel<E, T, F><<<grid, block, sm, st>>>(tb, p); } while (0)
-#define LAUNCH_F(E, T) do { if (fast) LAUNCH(E, T, true); else LAUNCH(E, T, false); } while (0)
+#define LAUNCH(E, T, F, W) do { set_smem(ofdm_demod_kernel<E, T, F, W>, sm); ofdm_demod_kernel<E, T, F, W><<<grid, block, sm, st>>>(tb, p); } while (0)
+#define LAUNCH_W(E, T, F) do { if (p.weighted) LAUNCH(E, T, F, true); else LAUNCH(E, T, F, false); } while (0)
+#define LAUNCH_F(E, T) do { if (fast) LAUNCH_W(E, T, true); else LAUNCH_W(E, T, false); } while (0)
     if (fft_mode == 0) { if (tap) LAUNCH_F(true, true); else LAUNCH_F(true, false); }
     else { if (tap) LAUNCH_F(false, true); else LAUNCH_F(false, false); }
 #undef LAUNCH_F
+#undef LAUNCH_W
 #undef LAUNCH
 }
 
@@ -986,8 +1025,8 @@ int ofdm_tail_frames(int n_frames)
     if (!resident) {
         int dev = 0, sms = 0, per_sm = 0;
         cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        set_smem(ofdm_demod_kernel<true, false, false>, sizeof(DemodSmem));
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ofdm_demod_kernel<true, false, false>, OFDM_THREADS, sizeof(DemodSmem));
+        set_smem(ofdm_demod_kernel<true, false, false, false>, sizeof(DemodSmem));
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ofdm_demod_kernel<true, false, false, false>, OFDM_THREADS, sizeof(DemodSmem));
         resident = sms * (per_sm > 0 ? per_sm : 1);
     }
     if (n_frames < 2 * resident) return 0;

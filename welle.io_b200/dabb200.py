@@ -18,6 +18,7 @@ SOFT_PER_FRAME = 75 * 3072
 MAX_SUBCH = 4
 FFT_EXACT, FFT_FMA = 0, 1
 NCO_EXACT, NCO_FAST = 0, 1
+DEMAP_REFERENCE, DEMAP_WEIGHTED = 0, 1
 IQ_CF32, IQ_U8, IQ_S8, IQ_S16LE, IQ_S16BE = 0, 1, 2, 3, 4
 FRAME_DECODED, FRAME_NEED_SAMPLES, FRAME_NO_SYNC, FRAME_ACQUIRING = 0, 1, 2, 3
 
@@ -35,6 +36,8 @@ class Config(C.Structure):
 
 class Options(C.Structure):
     _fields_ = [("disable_coarse", C.c_int32), ("fft_placement", C.c_int32), ("freqsync_method", C.c_int32), ("decode_tii", C.c_int32), ("count_bit_errors", C.c_int32), ("reserved", C.c_int32 * 3)]
+    # dabb_options.soft_demap is the C struct's former reserved[0]: the ctypes layout keeps the word inside `reserved`
+    soft_demap = property(lambda self: self.reserved[0], lambda self, v: self.reserved.__setitem__(0, v))
 
 
 PLACEMENT_THRESHOLD_BEFORE_PEAK, PLACEMENT_STRONGEST_PEAK, PLACEMENT_EARLIEST_PEAK_WITH_BINNING = 0, 1, 2
@@ -350,9 +353,11 @@ class Context:
         self._ck(self.lib.dabb_get_info(self.h, int(what), C.byref(v)))
         return v.value
 
-    def set_options(self, disable_coarse=True, fft_placement=0, freqsync_method=0, decode_tii=False, count_bit_errors=False):
+    def set_options(self, disable_coarse=True, fft_placement=0, freqsync_method=0, decode_tii=False, count_bit_errors=False, soft_demap=DEMAP_REFERENCE):
+        """soft_demap: DEMAP_REFERENCE (the reference's demap) or DEMAP_WEIGHTED (weak carriers scaled by their level over the symbol's
+        geometric-mean level, see dabb_options.soft_demap)"""
         o = Options(); o.disable_coarse, o.fft_placement, o.freqsync_method, o.decode_tii = int(disable_coarse), int(fft_placement), int(freqsync_method), int(decode_tii)
-        o.count_bit_errors = int(count_bit_errors)
+        o.count_bit_errors, o.soft_demap = int(count_bit_errors), int(soft_demap)
         self._ck(self.lib.dabb_set_options(self.h, C.byref(o)))
 
     def read_tap(self, what, stride=0):

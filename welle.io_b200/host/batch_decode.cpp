@@ -2,8 +2,8 @@
  * batch_decode.cpp — native batch driver over the C ABI: decodes many RAW IQ recordings at once, one stream per file (or per ensemble of a
  * wideband file, --rate), on one GPU.
  *
- *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--rate HZ --offset HZ[,HZ...]|auto]
- *                [--rate HZ --scan] --out DIR file1 [file2 ...]
+ *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference]
+ *                [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file1 [file2 ...]
  *
  * What `welle-cli -f FILE -D` does for one recording (welle-cli.cpp:215-235,612-707: dump the FIC, tune to the first audio
  * service, dump its logical frames) done for all files in lock-step: every iteration hands each stream's next window of samples
@@ -18,6 +18,11 @@
  *
  * --ber: channel bit errors counted on the device (dabb_options.count_bit_errors, tap 10); every decoded frame adds one line
  * "fic_bits fic_errors fic_erasures codewords bits errors erasures" to DIR/<name>.ber, the last four for the service's slot (0).
+ *
+ * --soft weighted|reference: the OFDM demodulator's soft-decision demap (dabb_options.soft_demap) of every context the driver creates,
+ * the --scan / --offset auto survey and confirmation contexts included.  reference (the default) is the reference decoder's demap and
+ * leaves the options untouched; weighted scales down the softbits of carriers below the symbol's geometric-mean level, which helps the
+ * Viterbi decoder in multipath (DABB_DEMAP_WEIGHTED).
  *
  * --rate HZ --offset HZ[,HZ...]: every file is a wideband recording at HZ samples/s (any rate dabb_chan_create accepts) and every offset
  * (Hz from the tuned frequency, may be negative) is one stream of the batch, decoded by a channelizer of the same context (dabb_chan_*):
@@ -305,8 +310,22 @@ bool run_wide(dabb_ctx* ctx, std::vector<Stream>& st, std::vector<Wide>& wf, int
 
 std::string base_name(const std::string& path) { const size_t slash = path.find_last_of('/'); return slash == std::string::npos ? path : path.substr(slash + 1); }
 
+/* a context of the scan with dabb_options.soft_demap = soft (--soft); the other options as cfg gives them; false on an error */
+static bool create_scan_ctx(const dabb_config& cfg, int soft, dabb_ctx** ctx)
+{
+    if (dabb_create(&cfg, ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return false; }
+    if (soft == DABB_DEMAP_REFERENCE) return true;
+    dabb_options op; memset(&op, 0, sizeof op);
+    op.disable_coarse = cfg.disable_coarse; op.fft_placement = cfg.fft_placement; op.freqsync_method = cfg.freqsync_method; op.soft_demap = soft;
+    if (dabb_set_options(*ctx, &op) == DABB_OK) return true;
+    fprintf(stderr, "batch_decode: %s\n", dabb_last_error(*ctx));
+    dabb_destroy(*ctx);
+    *ctx = nullptr;
+    return false;
+}
+
 /* --scan: the ensembles of every file (ascending offset, per file), as the streams of their confirmation decode; false on an error */
-bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int device, std::vector<std::vector<Stream>>& found)
+bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int device, int soft, std::vector<std::vector<Stream>>& found)
 {
     const int64_t TF = DABB_TF;
     const int bps = bytes_per_sample(fmt);
@@ -338,7 +357,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
     dabb_config cfg; memset(&cfg, 0, sizeof cfg);
     cfg.abi_version = DABB_ABI_VERSION; cfg.device = device; cfg.n_streams = 1; cfg.transmission_mode = 1;
     dabb_ctx* ctx = nullptr;
-    if (dabb_create(&cfg, &ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return false; }
+    if (!create_scan_ctx(cfg, soft, &ctx)) return false;
     std::vector<float> psd(files.size() * (size_t)nfft);
     dabb_survey_io sio; memset(&sio, 0, sizeof sio);
     sio.in = buf.data(); sio.in_is_host = 1; sio.iq_format = fmt; sio.in_stride = in_len; sio.n_inputs = (int32_t)files.size(); sio.nfft = nfft;
@@ -371,7 +390,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
         const int S = (int)cs.size();
         if (S == 0) return true;
         cfg.n_streams = S; cfg.disable_coarse = disable_coarse; cfg.freqsync_method = freqsync;
-        if (dabb_create(&cfg, &ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return false; }
+        if (!create_scan_ctx(cfg, soft, &ctx)) return false;
         dabb_stream_reset(ctx, 0, S, 0);
         Outputs o; o.res.resize((size_t)S); o.fibs.resize((size_t)S * 12 * 32);
         std::vector<int64_t> buf_start((size_t)S);
@@ -440,7 +459,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
 
 int main(int argc, char** argv)
 {
-    int fmt = DABB_IQ_CF32, device = 0; bool coarse = false, tii = false, ber = false; std::string out;
+    int fmt = DABB_IQ_CF32, device = 0, soft = DABB_DEMAP_REFERENCE; bool coarse = false, tii = false, ber = false; std::string out;
     int64_t rate = 0; std::vector<int64_t> offsets; bool scan_only = false, auto_offsets = false;
     std::vector<std::string> files;
     for (int i = 1; i < argc; i++) {
@@ -455,6 +474,11 @@ int main(int argc, char** argv)
         else if (a == "--coarse") coarse = true;
         else if (a == "--tii") tii = true;
         else if (a == "--ber") ber = true;
+        else if (a == "--soft" && i + 1 < argc) {
+            const std::string m = argv[++i];
+            soft = m == "reference" ? DABB_DEMAP_REFERENCE : m == "weighted" ? DABB_DEMAP_WEIGHTED : -1;
+            if (soft < 0) { fprintf(stderr, "unknown soft demap %s\n", m.c_str()); return 2; }
+        }
         else if (a == "--rate" && i + 1 < argc) rate = atoll(argv[++i]);
         else if (a == "--scan") scan_only = true;
         else if (a == "--offset" && i + 1 < argc && std::string(argv[i + 1]) == "auto") { auto_offsets = true; i++; }
@@ -470,7 +494,7 @@ int main(int argc, char** argv)
     }
     if (out.empty() || files.empty() || (rate > 0) != ((int)!offsets.empty() + (int)scan_only + (int)auto_offsets == 1)
         || (rate <= 0 && (scan_only || auto_offsets))) {
-        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
+        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
         return 2;
     }
     const bool wide = rate > 0;
@@ -478,7 +502,7 @@ int main(int argc, char** argv)
     std::vector<std::vector<int64_t>> file_offsets(wide ? files.size() : 0, offsets);
     if (scan_only || auto_offsets) {
         std::vector<std::vector<Stream>> found;
-        if (!scan(files, rate, fmt, device, found)) return 1;
+        if (!scan(files, rate, fmt, device, soft, found)) return 1;
         for (size_t f = 0; f < files.size(); f++) {
             file_offsets[f].clear();
             for (const Stream& z : found[f]) file_offsets[f].push_back(z.offset + z.corr);
@@ -512,9 +536,9 @@ int main(int argc, char** argv)
     cfg.disable_coarse = coarse ? 0 : 1; cfg.n_subch_slots = DABB_MAX_SUBCH; cfg.max_subch_cu = 416;
     dabb_ctx* ctx = nullptr;
     if (dabb_create(&cfg, &ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return 1; }
-    if (tii || ber) {
+    if (tii || ber || soft != DABB_DEMAP_REFERENCE) {
         dabb_options op; memset(&op, 0, sizeof op);
-        op.disable_coarse = cfg.disable_coarse; op.decode_tii = tii; op.count_bit_errors = ber;
+        op.disable_coarse = cfg.disable_coarse; op.decode_tii = tii; op.count_bit_errors = ber; op.soft_demap = soft;
         if (dabb_set_options(ctx, &op) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
     }
 
