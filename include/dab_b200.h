@@ -258,7 +258,10 @@ int dabb_profile(dabb_ctx* ctx, int32_t enable);
 int dabb_profile_read(dabb_ctx* ctx, char* json_out, size_t cap);
 
 /* taps (valid after a dabb_process when keep_taps=1):
- *   0 = softbits int8 [n_streams][75*3072]
+ *   0 = softbits int8 [n_streams][75*3072]               also without keep_taps.  Such a context demaps only the symbols its decoders
+ *                                                        read (the FIC's and each selected sub-channel's); reading tap 0 repeats the
+ *                                                        last step's OFDM launch over every symbol first, so the last step's input
+ *                                                        samples must still be in place
  *   1 = CIR float [n_streams][2048]                     RadioControllerInterface::onNewImpulseResponse (phasereference.cpp:93)
  *   2 = constellation cf32 [n_streams][75][16]          onConstellationPoints: r1 of every 96th carrier (ofdm-decoder.cpp:216-218)
  *   3 = null symbol cf32 [n_streams][2656], NCO applied  onNewNullSymbol (ofdm-processor.cpp:462-469)

@@ -150,6 +150,9 @@ struct dabb_ctx {
     std::vector<std::pair<std::string, std::pair<double, long>>> prof_acc;
     // spectrum survey (survey.cu), allocated by the first dabb_survey: twiddle and window tables, host input staging, per-chunk sums, spectra
     DevBuf<dabb_channel::cf> d_svy_tw; DevBuf<float> d_svy_win; DevBuf<uint8_t> d_svy_stage; DevBuf<float> d_svy_part, d_svy_psd;
+    // without keep_taps: [S][OFDM_MASK_WORDS] the OFDM symbols each stream's decoders read (ofdm_mask.cuh), rebuilt by every select and
+    // remove call; the OFDM launch of the last step, which tap 0 repeats over every symbol when soft_partial says it skipped some
+    DevBuf<uint32_t> d_symmask; OfdmParams soft_op{}; bool soft_partial = false;
 };
 
 namespace {
@@ -596,6 +599,25 @@ int repitch(dabb_ctx* ctx, DevBuf<uint8_t>& b, size_t rows, size_t old_pitch, si
     return DABB_OK;
 }
 
+// the symbol masks of streams [first, first + count) from their slots (h_slots), uploaded on the context's stream; the caller synchronises
+// it before the host vector is gone (the copy is from pageable memory, so it is staged before cudaMemcpyAsync returns anyway)
+int upload_symmask(dabb_ctx* ctx, int first, int count)
+{
+    if (!ctx->d_symmask) return DABB_OK;
+    const int ns = ctx->n_slots;
+    std::vector<uint32_t> m((size_t)count * OFDM_MASK_WORDS);
+    for (int i = 0; i < count; i++) {
+        OfdmMaskSlot sl[DABB_MAX_SUBCH];
+        for (int k = 0; k < ns; k++) {
+            const MscSlotState& st = ctx->h_slots[(size_t)(first + i) * ns + k];
+            sl[k] = OfdmMaskSlot{st.enabled, st.start_cu, st.frag / 64};
+        }
+        build_ofdm_mask(sl, ns, m.data() + (size_t)i * OFDM_MASK_WORDS);
+    }
+    CK(cudaMemcpyAsync(ctx->d_symmask + (size_t)first * OFDM_MASK_WORDS, m.data(), m.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    return DABB_OK;
+}
+
 // streams [first, first + count) of `slot` take state v (v.enabled = 0: removed).  The slot's grouped Viterbi schedule, its decision
 // buffer and its largest frame length follow the new membership; the new buffers are allocated and filled before any is replaced, so
 // that a failed allocation leaves the slot as it was.  Every other stream's state and buffers are untouched.  (The caller has run
@@ -628,6 +650,7 @@ int set_slot_streams(dabb_ctx* ctx, int slot, int first, int count, const MscSlo
     }
     set_slot_kernel<<<(count + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_slots, ns, slot, first, count, v);
     for (int i = first; i < first + count; i++) ctx->h_slots[(size_t)i * ns + slot] = v;
+    if ((rc = upload_symmask(ctx, first, count))) return rc;
     { int rc_ = check_launch(ctx, "set_slot_kernel"); cudaStreamSynchronize(ctx->stream); return rc_; }
 }
 
@@ -741,6 +764,8 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
     if (ctx->keep_taps && ((rc = dalloc(ctx, ctx->d_cir, (size_t)S * TU)) || (rc = dalloc(ctx, ctx->d_r1, (size_t)S * 75 * 1536)) || (rc = dalloc(ctx, ctx->d_null, (size_t)S * TNULL)))) return fail(rc);
     if ((rc = dalloc(ctx, ctx->d_dec, vit_dec_bytes(S * 4, 774) / sizeof(uint2), false)) || (rc = dalloc(ctx, ctx->d_dec_fic, vit_dec_bytes(S * 4, 774) / sizeof(uint2), false))) return fail(rc);
     ctx->h_slots.assign((size_t)S * ctx->n_slots, MscSlotState{});
+    // keep_taps exposes every symbol's softbits and constellation, so only a context without it skips the symbols nothing reads
+    if (!ctx->keep_taps && ((rc = dalloc(ctx, ctx->d_symmask, (size_t)S * OFDM_MASK_WORDS)) || (rc = upload_symmask(ctx, 0, S)))) return fail(rc);
     ctx->profiles.reserve(DABB_MAX_PROFILES);
     if ((rc = dalloc(ctx, ctx->d_profiles, DABB_MAX_PROFILES))) return fail(rc);
     // info arrays of unconfigured slots are never read (finalize skips disabled slots)
@@ -966,7 +991,9 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     op.r1 = ctx->d_r1; op.freqcorr = d_fc; op.level = d_lvl; op.snr = d_snr; op.n_frames = S; op.groups = ctx->groups; op.sym_per_cta = 75 / ctx->groups;
     op.trace = ctx->trace;
     op.n_full = S - ctx->tail_frames; op.tail_groups = ctx->tail_frames ? OFDM_TAIL_GROUPS : 1; op.fc_pitch = ctx->fc_pitch; op.nco_fast = ctx->nco_fast; op.weighted = ctx->soft_demap == DABB_DEMAP_WEIGHTED;
+    op.symmask = ctx->d_symmask;
     launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, A);
+    ctx->soft_op = op; ctx->soft_partial = op.symmask != nullptr;
     if ((rc = check_launch(ctx, "ofdm_demod_kernel"))) return rc;
     advance_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, S, ctx->fc_pitch, d_fc, d_lvl);
     if ((rc = check_launch(ctx, "advance_kernel"))) return rc;
@@ -1157,6 +1184,16 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
     if (!ctx || !host_out) return DABB_E_ARG;
     cudaSetDevice(ctx->device);
     sync_all(ctx);
+    if (what == 0 && ctx->soft_partial) {
+        // the last step demapped only the symbols its decoders read: repeat its OFDM launch over every symbol, from the same input and
+        // per-frame parameters, writing nothing but the softbits (the symbols it did demap get the same bytes again)
+        OfdmParams op = ctx->soft_op;
+        op.symmask = nullptr; op.r1 = nullptr; op.freqcorr = nullptr; op.level = nullptr; op.snr = nullptr; op.trace = TraceBuf{nullptr, nullptr, 0};
+        launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, ctx->stream);
+        CK(cudaGetLastError());
+        CK(cudaStreamSynchronize(ctx->stream));
+        ctx->soft_partial = false;
+    }
     if (what == 0) { const size_t n = (size_t)ctx->S * DABB_SOFT_PER_FRAME; CK(cudaMemcpy(host_out, ctx->d_soft + (size_t)ctx->last_parity * n, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 1 && ctx->d_cir) { const size_t n = (size_t)ctx->S * TU * 4; CK(cudaMemcpy(host_out, ctx->d_cir, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 2 && ctx->d_r1) {      // every 96th logical carrier of every data symbol (constellationDecimation, ofdm-decoder.h:87)

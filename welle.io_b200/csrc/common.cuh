@@ -7,6 +7,7 @@
 #include "tii_core.cuh"
 #include "ber_core.cuh"
 #include "chan_core.cuh"
+#include "ofdm_mask.cuh"
 
 namespace dabb {
 
@@ -58,6 +59,7 @@ struct OfdmParams {
     int fc_pitch;                                // freqcorr entries per frame (>= groups, tail_groups); 0 -> the larger of the two
     int nco_fast;                                // DABB_NCO_FAST: fp32 oscillator (tolerance mode)
     int weighted;                                // DABB_DEMAP_WEIGHTED: softbits against max(carrier level, the symbol's geometric-mean level)
+    const uint32_t* symmask;                     // [n][OFDM_MASK_WORDS] the symbols each frame demaps (ofdm_mask.cuh), or nullptr: all of them
     TraceBuf trace;                              // rec == nullptr: off
 };
 

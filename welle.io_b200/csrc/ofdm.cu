@@ -195,6 +195,16 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
+// one term of the fine-AFC correlation, fc += x conj(b), rounded as the contracted form the kernel always compiled to (so the transformed
+// and the light symbols of ofdm_demod_kernel round identically)
+__device__ __forceinline__ void afc_acc(float2& fc, float2 x, float2 b)
+{
+    fc.x = __fadd_rn(fc.x, __fmaf_rn(x.x, b.x, __fmul_rn(x.y, b.y)));
+    fc.y = __fadd_rn(fc.y, __fmaf_rn(x.y, b.x, -__fmul_rn(x.x, b.y)));
+}
+// |re| + |im| of a thread's first (mixed) window sample: the sub-sampled input of the running signal level (see advance_kernel)
+__device__ __forceinline__ float level_sample(float2 x) { return fabsf(x.x) + fabsf(x.y); }
+
 // (1 - 1e-5)^2552: what the reference's level tracker sLevel = 1e-5 |v|_1 + (1 - 1e-5) sLevel (ofdm-processor.cpp:166,215) forgets per symbol
 constexpr float LEVEL_DECAY_SYM = 0.97480279f;
 #ifndef DEMOD_CTAS_PER_SM
@@ -215,8 +225,62 @@ struct __align__(16) DemodSmem {
 #endif
     float2 rtab[2][16];              // DABB_NCO_FAST: e^{-j theta((128 h + 256 c) Hz)} for the PRS / the data symbols
     float red[16];
-    uint64_t full;
+    uint64_t full;                   // a transformed symbol's copy, or a light symbol's in the first half of inbuf
+    uint64_t half1;                  // a light symbol's copy in the second half of inbuf
+    uint8_t kind[NSYM];              // per symbol of the frame: SYM_LIGHT, SYM_FFT or SYM_DEMAP (from the frame's symbol mask)
 };
+
+// A symbol that no decoder reads and that is no demapped symbol's reference is "light": it contributes only its fine-AFC terms and its
+// level sample, which need the guard interval, the last T_g samples and the first OFDM_THREADS window samples - the symbol's samples
+// [0, LIGHT_A) and [T_u, T_s), 9.1 instead of 20.4 KB.  Two light symbols are staged at once, one in each half of inbuf: the first span
+// at the half's start, the second LIGHT_B samples later (each with the transformed symbol's 16-byte alignment shift).
+enum : uint8_t { SYM_LIGHT = 0, SYM_FFT = 1, SYM_DEMAP = 2 };
+constexpr int IN_HALF = IN_CAP / 2, LIGHT_A = TG + OFDM_THREADS, LIGHT_B = 640;
+static_assert(LIGHT_B >= LIGHT_A + 2 && LIGHT_B % 2 == 0 && LIGHT_B + TG + 2 <= IN_HALF, "light symbol staging");
+
+// a light symbol at lb (= the half's start + the alignment shift): exactly the per-thread fine-AFC terms and level sample the transformed
+// path (fft2048_from_smem) takes for it, in the same order and with the same oscillator phases; window sample n >= T_u - T_g is at
+// lb[LIGHT_B + n - (T_u - T_g)], its partner T_u earlier at lb[n - (T_u - T_g)], window sample t at lb[T_g + t]
+template <bool FASTNCO>
+__device__ __forceinline__ void light_symbol(const float2* lb, int64_t idx0, int t, const DevTables& tb, const Nco& nco, float2& fc, const float2* rtab, float& l1_first)
+{
+    const float2* tail = lb + LIGHT_B;
+    if (FASTNCO && nco.mix) {
+        // raw samples for the correlation (the frame's sum is rotated once at the end of the kernel)
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int c = 6; c < 8; c++) {
+                const int n = t + 128 * h + 256 * c;
+                if (n >= TU - TG) afc_acc(fc, tail[n - (TU - TG)], lb[n - (TU - TG)]);
+            }
+        const float2 o0 = osc_fast(mod_rate64((int64_t)nco.lp0 - (idx0 + t) * (int64_t)nco.ph));
+        l1_first = level_sample(cmul_fast(lb[TG + t], cmul_fast(o0, rtab[0])));
+        return;
+    }
+    if (nco.mix) {
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int c = 6; c < 8; c++) {
+                const int n = t + 128 * h + 256 * c;
+                if (n >= TU - TG) {
+                    const int32_t l = mod_rate64((int64_t)nco.lp0 - (idx0 + n) * (int64_t)nco.ph);
+                    afc_acc(fc, mix_sample(tail[n - (TU - TG)], tb, l), mix_sample(lb[n - (TU - TG)], tb, sub_mod(l, nco.u2048)));
+                }
+            }
+        l1_first = level_sample(mix_sample(lb[TG + t], tb, mod_rate64((int64_t)nco.lp0 - (idx0 + t) * (int64_t)nco.ph)));
+        return;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+        for (int c = 6; c < 8; c++) {
+            const int n = t + 128 * h + 256 * c;
+            if (n >= TU - TG) afc_acc(fc, tail[n - (TU - TG)], lb[n - (TU - TG)]);
+        }
+    l1_first = level_sample(lb[TG + t]);
+}
 
 // one symbol's samples, already in shared memory at in[0..], -> spectrum in registers (same pass structure as
 // fft2048_from_global); idx0 = frame-relative index of in[0] for the NCO phase
@@ -248,16 +312,12 @@ __device__ __forceinline__ void fft2048_from_smem(const float2* in, int64_t idx0
 #pragma unroll
                 for (int c = 6; c < 8; c++) {
                     const int n = t + 128 * h + 256 * c;
-                    if (n >= TU - TG) {
-                        const float2 b = in[n - TU];
-                        fc.x += x[c].x * b.x + x[c].y * b.y;
-                        fc.y += x[c].y * b.x - x[c].x * b.y;
-                    }
+                    if (n >= TU - TG) afc_acc(fc, x[c], in[n - TU]);
                 }
             }
 #pragma unroll
             for (int c = 0; c < 8; c++) x[c] = cmul_fast(x[c], cmul_fast(o0, rtab[8 * h + c]));
-            if (h == 0) l1_first = fabsf(x[0].x) + fabsf(x[0].y);
+            if (h == 0) l1_first = level_sample(x[0]);
             float2 y[8];
             passA_block<EXACT, false>(x, y, twp);
 #pragma unroll
@@ -281,11 +341,7 @@ __device__ __forceinline__ void fft2048_from_smem(const float2* in, int64_t idx0
                 x[c] = mix_sample(x[c], tb, l);
                 if (c >= 6 && afc) {
                     const int n = t + 128 * h + 256 * c;
-                    if (n >= TU - TG) {
-                        const float2 b = mix_sample(in[n - TU], tb, sub_mod(l, nco.u2048));     // phase of the sample T_u earlier
-                        fc.x += x[c].x * b.x + x[c].y * b.y;
-                        fc.y += x[c].y * b.x - x[c].x * b.y;
-                    }
+                    if (n >= TU - TG) afc_acc(fc, x[c], mix_sample(in[n - TU], tb, sub_mod(l, nco.u2048)));     // phase of the sample T_u earlier
                 }
                 l = sub_mod(l, nco.d256);
             }
@@ -293,14 +349,10 @@ __device__ __forceinline__ void fft2048_from_smem(const float2* in, int64_t idx0
 #pragma unroll
             for (int c = 6; c < 8; c++) {
                 const int n = t + 128 * h + 256 * c;
-                if (n >= TU - TG) {
-                    const float2 b = in[n - TU];
-                    fc.x += x[c].x * b.x + x[c].y * b.y;
-                    fc.y += x[c].y * b.x - x[c].x * b.y;
-                }
+                if (n >= TU - TG) afc_acc(fc, x[c], in[n - TU]);
             }
         }
-        if (h == 0) l1_first = fabsf(x[0].x) + fabsf(x[0].y);
+        if (h == 0) l1_first = level_sample(x[0]);
         float2 y[8];
         passA_block<EXACT, false>(x, y, twp);
 #pragma unroll
@@ -341,7 +393,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
     DemodSmem& sm = *reinterpret_cast<DemodSmem*>(smraw);
     const int t = threadIdx.x;
     // ---- once per CTA
-    if (t == 0) { mbar_init(&sm.full, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+    if (t == 0) { mbar_init(&sm.full, 1); if (!TAP) mbar_init(&sm.half1, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 #if DEMOD_SLIM
     uint16_t* const sbuf = reinterpret_cast<uint16_t*>(sm.xbuf);
 #else
@@ -359,7 +411,6 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
     // (bits 0-7 / 8-15: slot, bit 16 / 17: halves stored swapped)
     const int rslot = t < 96 ? (((int)tb.invperm[2 * TU + t] & 0xFF) | (((int)tb.invperm[2 * TU + t + 96] & 0xFF) << 8) |
                                (((int)tb.invperm[2 * TU + t] >> 8) << 16) | (((int)tb.invperm[2 * TU + t + 96] >> 8) << 17)) : 0;
-    uint32_t parity = 0;
     __syncthreads();
 
     // One CTA per work item: the first n_full frames are walked by `groups` items each; the remaining (tail) frames are cut into
@@ -387,7 +438,23 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
         mbar_expect_tx(&sm.full, bytes);
         bulk_g2s(sm.inbuf, g0 - shift, bytes, &sm.full);
     };
-    if (t == 0) issue(l_first - 1);
+    // a light symbol (l >= 1) into half h of inbuf: its samples [0, LIGHT_A) and [T_u, T_s), on that half's barrier
+    auto issue_light = [&](int l, int h) {
+        const float2* g0 = src + (int64_t)TU + (int64_t)(l - 1) * TS;
+        const int shift = (int)((reinterpret_cast<uintptr_t>(g0) >> 3) & 1);
+        const uint32_t ba = (uint32_t)(((LIGHT_A + shift + 1) & ~1) * 8), bb = (uint32_t)(((TG + shift + 1) & ~1) * 8);
+        uint64_t* bar = h ? &sm.half1 : &sm.full;
+        mbar_expect_tx(bar, ba + bb);
+        bulk_g2s(sm.inbuf + IN_HALF * h, g0 - shift, ba, bar);
+        bulk_g2s(sm.inbuf + IN_HALF * h + LIGHT_B, g0 + TU - shift, bb, bar);
+    };
+    // what each symbol of the frame needs (CTA-uniform): transformed when it is the phase reference symbol, demapped, or the reference of
+    // a demapped symbol; light otherwise.  No mask: every symbol is transformed and demapped.
+    if (!TAP && t < NSYM) {
+        const uint32_t* m = p.symmask ? p.symmask + (int64_t)f * OFDM_MASK_WORDS : nullptr;
+        const bool dm = !m || ((m[t >> 5] >> (t & 31)) & 1u), dm1 = !m || (t + 1 < NSYM && ((m[(t + 1) >> 5] >> ((t + 1) & 31)) & 1u));
+        sm.kind[t] = (t > 0 && dm) ? SYM_DEMAP : ((t == 0 || dm1) ? SYM_FFT : SYM_LIGHT);
+    }
 
     // nco[f] = {phase applied to PRS sample 0, Hz for the PRS, phase at index 0 extrapolated for the data symbols, Hz}
     const Nco ncoP = make_nco(p.nco ? p.nco[4 * f] : 0, p.nco ? p.nco[4 * f + 1] : 0);
@@ -397,31 +464,62 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
         const int k = t & 15;
         sm.rtab[t >> 4][k] = osc_fast(mod_rate64(-(int64_t)(128 * (k >> 3) + 256 * (k & 7)) * n.ph));
     }
-    if (FASTNCO) __syncthreads();
+    if (FASTNCO || !TAP) __syncthreads();
+
+    // Staging: inbuf holds one transformed symbol or two light ones.  Symbols are copied in order, each as soon as its space is free
+    // (a transformed one needs both halves); light symbols alternate between the halves.  The reference symbol l_first - 1 of a later
+    // item is staged only when it is transformed: a light one contributes nothing to this item.
+    // (the TAP instances always run without a mask: every symbol is transformed)
+    auto kind_of = [&](int l) -> int { return TAP ? (l ? SYM_DEMAP : SYM_FFT) : sm.kind[l]; };
+    const int l_begin = (l_first > 1 && kind_of(l_first - 1) == SYM_LIGHT) ? l_first : l_first - 1;
+    int nxt = l_begin;                    // next symbol to copy
+    int used = 0, ih = 0, ch = 0;         // halves in use; half of the next light copy, of the next light symbol to consume
+    uint32_t parity = 0;                  // bit h: phase parity of the barrier of half h (half 0's is also the transformed symbols')
+    auto fill = [&]() {
+        while (nxt < l_last) {
+            const int need = kind_of(nxt) == SYM_LIGHT ? 1 : 2;
+            if (used + need > 2) break;
+            if (t == 0) {
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                if (need == 2) issue(nxt); else issue_light(nxt, ih);
+            }
+            if (need == 1) ih ^= 1;
+            used += need; nxt++;
+        }
+    };
+    fill();
 
     float2 prev[NSLOT];
     float2 fc = make_float2(0.f, 0.f);
     float lvl = 0.f;                                  // decayed sum of one sample magnitude per symbol and thread (signal level estimate)
 
-    for (int l = l_first - 1; l < l_last; l++) {
+    for (int l = l_begin; l < l_last; l++) {
         const int64_t s0 = (l == 0) ? 0 : (int64_t)TU + (int64_t)(l - 1) * TS;
         const int goff = (l == 0) ? 0 : TG;
         const int shift = (int)((reinterpret_cast<uintptr_t>(src + s0) >> 3) & 1);
+        const int kind = kind_of(l);
+        if (kind == SYM_LIGHT) {               // l >= l_first: its fine-AFC terms and level sample only
+            mbar_wait(ch ? &sm.half1 : &sm.full, (parity >> ch) & 1); parity ^= 1u << ch;
+            float l1s;
+            light_symbol<FASTNCO>(sm.inbuf + IN_HALF * ch + shift, s0 + TG, t, tb, ncoS, fc, sm.rtab[1], l1s);
+            lvl = fmaf(lvl, LEVEL_DECAY_SYM, l1s);
+            ch ^= 1;
+            __syncthreads();                   // the half is consumed
+            used -= 1; fill();
+            continue;
+        }
         const Nco& nco = l == 0 ? ncoP : ncoS;
-        mbar_wait(&sm.full, parity); parity ^= 1;
+        mbar_wait(&sm.full, parity & 1); parity ^= 1;
         const float2* in = sm.inbuf + shift;
         float2 v[16];
         float l1s;
         fft2048_from_smem<EXACT, FASTNCO>(in + goff, s0 + goff, v, sm, t, xi, tw_c5, tb, nco, l >= l_first, fc, sm.rtab[l == 0 ? 0 : 1], l1s);
         if (l >= l_first || l == 0) lvl = fmaf(lvl, LEVEL_DECAY_SYM, l1s);
         __syncthreads();                       // (1) inbuf fully consumed, pass-A results in xbuf
-        if (t == 0 && l + 1 < l_last) {        // prefetch the next symbol while passes B, C and the demap run
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            issue(l + 1);
-        }
+        used = 0; fill();                      // prefetch the next symbol(s) while passes B, C and the demap run
         fft2048_finish<EXACT>(v, sm, t, xi, tw_c5, b2);   // contains barrier (2)
 
-        if (l >= l_first) {
+        if (l >= l_first && kind == SYM_DEMAP) {
             if (WEIGHTED) {
                 // DABB_DEMAP_WEIGHTED: r1 of every owned bin into v[] (its spectrum moves to prev[]), the symbol's geometric-mean carrier
                 // level G from one block reduction, then the demap against max(l1, G) (ofdm_core.cuh: level_acc, level_gmean)
@@ -477,7 +575,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
             __syncthreads();        // staging area read: the next symbol's first pass may overwrite the exchange buffer
 #endif
         } else {
-            // reference symbol only (the PRS when l == 0): keep its spectrum, estimate SNR from the PRS
+            // a reference only (the PRS when l == 0, or a symbol no decoder reads before one they do): keep its spectrum, estimate SNR from the PRS
 #pragma unroll
             for (int s = 0; s < NSLOT; s++) prev[s] = v[slot_c(s)];
             __syncthreads();                   // (3') every thread is done reading xbuf before the next symbol's pass A overwrites it
