@@ -84,7 +84,9 @@ typedef struct {
     int32_t count_bit_errors;   /* count the channel bit errors of the FIC and of every decoded sub-channel codeword on the device (tap 10) */
     int32_t soft_demap;         /* DABB_DEMAP_*: how the OFDM demodulator turns each carrier into softbits (see below); a value outside the
                                    enum is refused with DABB_E_ARG and the call changes nothing */
-    int32_t reserved[2];
+    int32_t sample_clock;       /* DABB_CLOCK_*: track each stream's sample-clock error and remove the phase ramp it puts on the softbits
+                                   (see below); a value outside the enum is refused with DABB_E_ARG and the call changes nothing */
+    int32_t reserved[1];
 } dabb_options;
 
 /* Soft-decision demap of the OFDM demodulator, dabb_options.soft_demap; takes effect from the next step, and dabb_ofdm_demod uses the
@@ -103,6 +105,37 @@ typedef struct {
  * both modes.  The FIC, MSC, BER and TII paths read the softbits unchanged; more softbits truncate to 0, so tap 10 counts more
  * erasures. */
 enum { DABB_DEMAP_REFERENCE = 0, DABB_DEMAP_WEIGHTED = 1 };
+
+/* Sample-clock tracking, dabb_options.sample_clock; takes effect from the next step.
+ * A recording whose sample clock is off by eps holds 2.048 M (1 + eps) samples per second of air time (ppm > 0: more samples).  Each
+ * symbol's FFT window then slips eps T_s samples against its symbol, which rotates the differential product r1 of carrier k by
+ * -2 pi k eps T_s / T_u (17 degrees at the band edge at 50 ppm; the DQPSK decision margin is 45).  Every frame is re-synchronised
+ * from its own phase reference symbol, so nothing fails visibly: the edge carriers just feed the Viterbi decoder partly wrong softbits.
+ * DABB_CLOCK_OFF (0, the default): nothing is estimated or derotated.
+ * DABB_CLOCK_TRACK (1) (replaces: none; the reference has no sample-clock correction) estimates eps per stream from its frame timing:
+ * a frame placed by the time synchronisation ends T_F eps samples later than the one before it, so over frames start_index - 504
+ * averages to T_F eps.  Per stream the estimate e (ppm, double), a count n of frames counted, and a flag "the previous active step
+ * decoded a frame" are kept.  In a step that decodes a frame (DABB_FRAME_DECODED) with TRACK:
+ *   d = start_index - 504; the frame counts when the flag is set and |d| <= 64 (325 ppm; larger values are placement jumps);
+ *   a counting frame does n = n + 1 (saturating), e = e + (1e6 d / 196608 - e) / min(n, 32)  (a running mean over the first 32 counted
+ *   frames, then an exponential average of 32 frames); the flag is set after every decoded frame.
+ * A step with DABB_FRAME_NO_SYNC or DABB_FRAME_ACQUIRING, or run with the option OFF, clears the flag; DABB_FRAME_NEED_SAMPLES changes
+ * nothing; a sync loss keeps e and n (the clock belongs to the recording), dabb_stream_reset clears all three, switching to OFF keeps
+ * e and n.  A frame is derotated with applied = (n >= 8 ? e : 0) from before the frame: for data symbol l >= 1 and carrier k
+ * (FFT bin k for k > 0, 2048 + k for k < 0) the demap reads
+ *   r1' = r1 exp(+2 pi i k applied 1e-6 T_s / T_u)
+ * with a phasor within 2^-22 of the exact value in each component, computed the same way whatever the launch configuration; the
+ * reference or weighted demap then runs on r1' (the weighted mode's G comes from the derotated levels).  applied == 0 leaves r1
+ * untouched, so the softbits are bit-identical to OFF.  r1_out (tap 2's constellation) holds the derotated products, the values the
+ * demap read.  Taps 0 and 11 and the FIC, MSC, BER and TII paths read the step's own values. */
+enum { DABB_CLOCK_OFF = 0, DABB_CLOCK_TRACK = 1 };
+/* one stream in one step: tap 11 (all zero when the step ran with sample_clock OFF) */
+typedef struct {
+    float ppm;                  /* (float)e after the step */
+    float applied_ppm;          /* the value this step's frame was derotated with (0 when no frame was decoded) */
+    int32_t frames;             /* n */
+    int32_t reserved;
+} dabb_clock_result;
 
 /* Channel bit errors of one stream in one step: tap 10, while dabb_options.count_bit_errors is set.  Per codeword (a FIC block of 768
  * bits, or a logical frame of 24 * bitrate bits) the decoded bits before energy dispersal (the output bytes MSB first, XOR the PRBS; 6
@@ -276,7 +309,9 @@ int dabb_profile_read(dabb_ctx* ctx, char* json_out, size_t cap);
  *   9 = dabb_tii_result [n_streams] of the last step (all zero when that step ran with decode_tii off); DABB_E_STATE until
  *       dabb_options.decode_tii has been set once
  *  10 = dabb_ber_result [n_streams] of the last step (all zero when that step ran with count_bit_errors off); DABB_E_STATE until
- *       dabb_options.count_bit_errors has been set once */
+ *       dabb_options.count_bit_errors has been set once
+ *  11 = dabb_clock_result [n_streams] of the last step (all zero when that step ran with sample_clock OFF); DABB_E_STATE until
+ *       dabb_options.sample_clock has been set to DABB_CLOCK_TRACK once */
 int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes);
 
 /* ---------------------------------------------------------------------------------------------------------
@@ -388,6 +423,10 @@ int dabb_survey_candidates(const float* psd, int32_t nfft, int64_t rate_hz, floa
  * The softbits follow the context's dabb_options.soft_demap (DABB_DEMAP_*); r1_out does not depend on it. */
 int dabb_ofdm_demod(dabb_ctx* ctx, const float* iq, int64_t stride_samples, const int64_t* prs_start, int32_t n_frames,
                     const int32_t* nco, int8_t* soft_out, float* r1_out, float* freqcorr_out);
+/* the same, with frame f derotated by clock_ppm[f] (device float [n], or NULL: none) as DABB_CLOCK_TRACK derotates a frame with its
+ * applied value; r1_out holds the derotated products.  NULL is exactly dabb_ofdm_demod; zeros give the same bits. */
+int dabb_ofdm_demod_ex(dabb_ctx* ctx, const float* iq, int64_t stride_samples, const int64_t* prs_start, int32_t n_frames,
+                       const int32_t* nco, const float* clock_ppm, int8_t* soft_out, float* r1_out, float* freqcorr_out);
 
 /* PhaseReference::findIndex, ThresholdBeforePeak (phasereference.cpp:73-97,212-253) for n windows of 2048 samples
  * at iq + f*stride + win_start[f]; index_out int32[n]; cir_out (may be NULL) float [n][2048] */

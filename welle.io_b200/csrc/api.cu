@@ -29,6 +29,7 @@ struct StreamState {
     float slevel;
     int32_t start_index;    // last findIndex
     int64_t nframes;
+    dabb_clock::State clk;  // sample-clock estimate (DABB_CLOCK_TRACK, clock_core.cuh): kept through a sync loss, cleared by dabb_stream_reset
 };
 
 struct StepScratch {        // per stream, rewritten every step
@@ -144,6 +145,9 @@ struct dabb_ctx {
     } pend[2], pend_sync;     // the two dabb_submit slots; dabb_process and taps 7 / 8, which never leave a step outstanding
     int pend_head = 0, pend_count = 0; int64_t submits = 0;
     int groups = 1; int fc_pitch = 1; int tail_frames = 0; int nco_fast = 0; int soft_demap = DABB_DEMAP_REFERENCE;
+    // sample-clock tracking, allocated when sample_clock is first set to TRACK: [2][S] the ppm each frame of a step is derotated with
+    // (double buffered by step parity, like the other per-step scratch) and the step's records (tap 11)
+    int sample_clock = DABB_CLOCK_OFF; DevBuf<float> d_clock_frame; DevBuf<dabb_clock_result> d_clock_res;
     DevBuf<const int32_t*> d_info_tab;
     // optional per-kernel timing: one event after every launch, durations = differences of consecutive events
     bool prof = false; std::vector<cudaEvent_t> prof_ev; std::vector<const char*> prof_name; size_t prof_used = 0;
@@ -299,7 +303,9 @@ __global__ void plan_kernel(StreamState* st, StepScratch* scr, const int64_t* bu
     win[s] = c.win_start; nco_sync[2 * s] = c.nco_sync[0]; nco_sync[2 * s + 1] = c.nco_sync[1]; active[s] = c.active;
 }
 
-__global__ void post_sync_kernel(StreamState* st, StepScratch* scr, const int32_t* index, const int32_t* coarse_corr, int S, int64_t* prs, int32_t* nco_frame, int32_t* active)
+// clock_frame (DABB_CLOCK_TRACK, else nullptr): the ppm the OFDM kernel derotates the frame with, the estimate from before the frame
+__global__ void post_sync_kernel(StreamState* st, StepScratch* scr, const int32_t* index, const int32_t* coarse_corr, int S, int64_t* prs, int32_t* nco_frame, int32_t* active,
+                                 float* clock_frame)
 {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= S) return;
@@ -332,16 +338,30 @@ __global__ void post_sync_kernel(StreamState* st, StepScratch* scr, const int32_
     scr[s] = c; st[s] = z;
     prs[s] = c.prs_start;
     nco_frame[4 * s] = lp_prs0; nco_frame[4 * s + 1] = p1; nco_frame[4 * s + 2] = lp_sym0; nco_frame[4 * s + 3] = p2;
+    if (clock_frame) clock_frame[s] = (float)dabb_clock::applied(z.clk);
 }
 
 // lane A, right after the OFDM kernel: the part of OFDMProcessor::run that feeds the next frame's synchronisation
 // (fine corrector update :450-451, consumed samples, NCO phase, corrector wrap :478-486)
-__global__ void advance_kernel(StreamState* st, StepScratch* scr, int S, int groups /* partial sums per frame */, const float2* fc_part, const float* lvl_part)
+// clock_track: the sample-clock estimator counts this step's frame (clock_core.cuh); clk_res (tap 11, or nullptr): the step's records
+__global__ void advance_kernel(StreamState* st, StepScratch* scr, int S, int groups /* partial sums per frame */, const float2* fc_part, const float* lvl_part,
+                               int clock_track, dabb_clock_result* clk_res)
 {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= S) return;
     StepScratch c = scr[s];
     StreamState z = st[s];
+    // sample clock: a decoded frame updates the estimate (with the value post_sync_kernel handed the demodulator recorded first); a step
+    // without sync, or with the option off, breaks the chain of consecutive frames; NEED_SAMPLES leaves it
+    dabb_clock_result cr{};
+    const bool clk_break = z.clk.prev && (!clock_track || c.status == DABB_FRAME_NO_SYNC || c.status == DABB_FRAME_ACQUIRING);
+    if (clock_track && c.active) {
+        cr.applied_ppm = (float)dabb_clock::applied(z.clk);
+        dabb_clock::update(z.clk, z.start_index);
+    }
+    if (clk_break) { z.clk.prev = 0; if (!c.active) st[s].clk.prev = 0; }
+    if (clock_track) { cr.ppm = (float)z.clk.e; cr.frames = z.clk.n; }
+    if (clk_res) clk_res[s] = cr;
     c.r_start_index = z.start_index; c.r_fx = 0.f; c.r_fy = 0.f;
     c.r_acq_failed = z.acq_failed;
     if (z.acq_failed) { z.acq_failed = 0; if (!c.active) st[s].acq_failed = 0; }
@@ -985,17 +1005,19 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         launch_find_index(ctx->dev, sp, ctx->fft_mode, A, 2);
         if ((rc = check_launch(ctx, "find_coarse_kernel"))) return rc;
     }
-    post_sync_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, d_index, ctx->disable_coarse ? nullptr : ctx->d_coarse.get(), S, d_prs, d_nco_frame, d_active);
+    const bool track = ctx->sample_clock == DABB_CLOCK_TRACK;
+    float* d_clock_frame = track ? ctx->d_clock_frame + (size_t)par * S : nullptr;
+    post_sync_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, d_index, ctx->disable_coarse ? nullptr : ctx->d_coarse.get(), S, d_prs, d_nco_frame, d_active, d_clock_frame);
     if ((rc = check_launch(ctx, "post_sync_kernel"))) return rc;
     OfdmParams op{}; op.iq = iq; op.stride = stride; op.prs_start = d_prs; op.nco = d_nco_frame; op.active = d_active; op.soft = d_soft; op.soft_stride = DABB_SOFT_PER_FRAME;
     op.r1 = ctx->d_r1; op.freqcorr = d_fc; op.level = d_lvl; op.snr = d_snr; op.n_frames = S; op.groups = ctx->groups; op.sym_per_cta = 75 / ctx->groups;
     op.trace = ctx->trace;
     op.n_full = S - ctx->tail_frames; op.tail_groups = ctx->tail_frames ? OFDM_TAIL_GROUPS : 1; op.fc_pitch = ctx->fc_pitch; op.nco_fast = ctx->nco_fast; op.weighted = ctx->soft_demap == DABB_DEMAP_WEIGHTED;
-    op.symmask = ctx->d_symmask;
+    op.symmask = ctx->d_symmask; op.clock = d_clock_frame;
     launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, A);
     ctx->soft_op = op; ctx->soft_partial = op.symmask != nullptr;
     if ((rc = check_launch(ctx, "ofdm_demod_kernel"))) return rc;
-    advance_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, S, ctx->fc_pitch, d_fc, d_lvl);
+    advance_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, S, ctx->fc_pitch, d_fc, d_lvl, track, ctx->d_clock_res.get());
     if ((rc = check_launch(ctx, "advance_kernel"))) return rc;
     // the null symbol: tap 3 with keep_taps, else (TII only) an internal buffer
     float2* d_null = ctx->d_null ? ctx->d_null.get() : (ctx->decode_tii ? ctx->d_tii_null.get() : nullptr);
@@ -1210,6 +1232,10 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
         if (!ctx->d_ber_res) { ctx->err = "tap 10 needs dabb_options.count_bit_errors to have been set"; return DABB_E_STATE; }
         const size_t n = sizeof(dabb_ber_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_ber_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
     }
+    if (what == 11) {
+        if (!ctx->d_clock_res) { ctx->err = "tap 11 needs dabb_options.sample_clock to have been set"; return DABB_E_STATE; }
+        const size_t n = sizeof(dabb_clock_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_clock_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
+    }
     if (what == 4 && ctx->d_tii && ctx->d_null && ctx->decode_tii) { const size_t n = (size_t)ctx->S * 2 * TU * 8; CK(cudaMemcpy(host_out, ctx->d_tii, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 3 && ctx->d_null) { const size_t n = (size_t)ctx->S * TNULL * 8; CK(cudaMemcpy(host_out, ctx->d_null, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 5) { const size_t n = sizeof(dabb_frame_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_results, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
@@ -1229,12 +1255,19 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
 // ------------------------------------------------------------------------------------------------ stage-level API
 int dabb_ofdm_demod(dabb_ctx* ctx, const float* iq, int64_t stride, const int64_t* prs_start, int32_t n, const int32_t* nco, int8_t* soft, float* r1, float* fc)
 {
+    return dabb_ofdm_demod_ex(ctx, iq, stride, prs_start, n, nco, nullptr, soft, r1, fc);
+}
+
+int dabb_ofdm_demod_ex(dabb_ctx* ctx, const float* iq, int64_t stride, const int64_t* prs_start, int32_t n, const int32_t* nco, const float* clock_ppm,
+                       int8_t* soft, float* r1, float* fc)
+{
     if (!ctx || !iq || !prs_start || !soft || n < 1) return DABB_E_ARG;
     cudaSetDevice(ctx->device);
     sync_all(ctx);
     OfdmParams op{}; op.iq = reinterpret_cast<const float2*>(iq); op.stride = stride; op.prs_start = prs_start; op.active = nullptr; op.soft = soft; op.soft_stride = DABB_SOFT_PER_FRAME;
     op.r1 = reinterpret_cast<float2*>(r1); op.freqcorr = reinterpret_cast<float2*>(fc); op.snr = nullptr; op.n_frames = n;
     op.groups = (fc || n >= 1024) ? 1 : (n >= 64 ? 5 : 25); op.sym_per_cta = 75 / op.groups; op.n_full = n; op.tail_groups = 1; op.fc_pitch = op.groups; op.nco_fast = ctx->nco_fast; op.weighted = ctx->soft_demap == DABB_DEMAP_WEIGHTED;
+    op.clock = clock_ppm;
     DevBuf<int32_t> nco4;
     int rc;
     if (nco) {
@@ -1297,7 +1330,8 @@ int dabb_get_info(dabb_ctx* ctx, int32_t what, int64_t* out)
 int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
 {
     if (!ctx || !opt || opt->fft_placement < 0 || opt->fft_placement > 2 || opt->freqsync_method < 0 || opt->freqsync_method > 2
-        || (opt->soft_demap != DABB_DEMAP_REFERENCE && opt->soft_demap != DABB_DEMAP_WEIGHTED)) return DABB_E_ARG;
+        || (opt->soft_demap != DABB_DEMAP_REFERENCE && opt->soft_demap != DABB_DEMAP_WEIGHTED)
+        || (opt->sample_clock != DABB_CLOCK_OFF && opt->sample_clock != DABB_CLOCK_TRACK)) return DABB_E_ARG;
     if (opt->decode_tii && !ctx->d_tii_res) {       // first use of TII: its buffers (64 KB per stream), zeroed = no open combinations
         cudaSetDevice(ctx->device);
         sync_all(ctx);
@@ -1324,8 +1358,16 @@ int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
         if ((rc = dalloc(ctx, ctx->d_ber_res, (size_t)ctx->S))) { ctx->d_ber_prof.reset(); return rc; }      // last: it marks the count as available
         CK(cudaStreamSynchronize(ctx->stream));
     }
+    if (opt->sample_clock == DABB_CLOCK_TRACK && !ctx->d_clock_res) {     // first use of clock tracking: the per-frame ppm and the records
+        cudaSetDevice(ctx->device);
+        sync_all(ctx);
+        int rc;
+        if ((rc = dalloc(ctx, ctx->d_clock_frame, 2 * (size_t)ctx->S))) return rc;
+        if ((rc = dalloc(ctx, ctx->d_clock_res, (size_t)ctx->S))) { ctx->d_clock_frame.reset(); return rc; }      // last: it marks tracking as available
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
     ctx->disable_coarse = opt->disable_coarse != 0; ctx->placement = opt->fft_placement; ctx->freqsync = opt->freqsync_method; ctx->decode_tii = opt->decode_tii != 0;
-    ctx->count_ber = opt->count_bit_errors != 0; ctx->soft_demap = opt->soft_demap;
+    ctx->count_ber = opt->count_bit_errors != 0; ctx->soft_demap = opt->soft_demap; ctx->sample_clock = opt->sample_clock;
     return DABB_OK;
 }
 

@@ -8,6 +8,7 @@
 #include "ber_core.cuh"
 #include "chan_core.cuh"
 #include "ofdm_mask.cuh"
+#include "clock_core.cuh"
 
 namespace dabb {
 
@@ -61,6 +62,7 @@ struct OfdmParams {
     int weighted;                                // DABB_DEMAP_WEIGHTED: softbits against max(carrier level, the symbol's geometric-mean level)
     const uint32_t* symmask;                     // [n][OFDM_MASK_WORDS] the symbols each frame demaps (ofdm_mask.cuh), or nullptr: all of them
     TraceBuf trace;                              // rec == nullptr: off
+    const float* clock;                          // [n] sample-clock ppm whose phase ramp the demap removes (clock_core.cuh), or nullptr: none
 };
 
 struct SyncParams {

@@ -237,6 +237,10 @@ struct __align__(16) DemodSmem {
 enum : uint8_t { SYM_LIGHT = 0, SYM_FFT = 1, SYM_DEMAP = 2 };
 constexpr int IN_HALF = IN_CAP / 2, LIGHT_A = TG + OFDM_THREADS, LIGHT_B = 640;
 static_assert(LIGHT_B >= LIGHT_A + 2 && LIGHT_B % 2 == 0 && LIGHT_B + TG + 2 <= IN_HALF, "light symbol staging");
+// sample-clock derotation (the CLOCK instances): the frame's factors Q[1..6] of dabb_clock::phasor live in the six entries of inbuf past
+// the largest copy (a transformed symbol: T_s samples + the alignment shift, rounded up to an even count), which no copy writes
+constexpr int CLK_Q = TS + 2;
+static_assert(CLK_Q + 6 <= IN_CAP, "clock factors behind the symbol copy");
 
 // a light symbol at lb (= the half's start + the alignment shift): exactly the per-thread fine-AFC terms and level sample the transformed
 // path (fft2048_from_smem) takes for it, in the same order and with the same oscillator phases; window sample n >= T_u - T_g is at
@@ -385,7 +389,7 @@ __device__ __forceinline__ void fft2048_finish(float2 v[16], DemodSmem& sm, int 
 #endif
 }
 
-template <bool EXACT, bool TAP, bool FASTNCO, bool WEIGHTED>
+template <bool EXACT, bool TAP, bool FASTNCO, bool WEIGHTED, bool CLOCK>
 __global__ void __launch_bounds__(OFDM_THREADS, DEMOD_CTAS_PER_SM)
 ofdm_demod_kernel(DevTables tb, OfdmParams p)
 {
@@ -465,6 +469,25 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
         sm.rtab[t >> 4][k] = osc_fast(mod_rate64(-(int64_t)(128 * (k >> 3) + 256 * (k & 7)) * n.ph));
     }
     if (FASTNCO || !TAP) __syncthreads();
+    // CLOCK: the frame's ppm (CTA-uniform); 0 leaves r1 untouched.  Carrier k = t + 128 j of this thread is derotated by P * Q[j]
+    // (dabb_clock::phasor): P in registers, Q[1..6] in shared memory, written here and first read after barrier (1) of the first symbol
+    float2 ckp = make_float2(1.f, 0.f);
+    bool rot = false;
+    if (CLOCK) {
+        const float a = p.clock[f];
+        rot = a != 0.f;
+        if (rot) {
+            ckp = dabb_clock::factor_p(t, a);
+            if (t < 6) sm.inbuf[CLK_Q + t] = dabb_clock::factor_q(t + 1, a);
+        }
+    }
+    // the phasor of slot s: bin t + 128 slot_c(s), carrier j = slot_c(s) (< 7) or slot_c(s) - 16
+    auto clk_phasor = [&](int s) -> float2 {
+        const int c = slot_c(s), j = c < 7 ? c : c - 16;
+        if (j == 0) return ckp;
+        const float2 q = sm.inbuf[CLK_Q - 1 + (j < 0 ? -j : j)];
+        return dabb_clock::cmul(ckp, j < 0 ? make_float2(q.x, -q.y) : q);
+    };
 
     // Staging: inbuf holds one transformed symbol or two light ones.  Symbols are copied in order, each as soon as its space is free
     // (a transformed one needs both halves); light symbols alternate between the halves.  The reference symbol l_first - 1 of a later
@@ -528,6 +551,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
                 for (int s = 0; s < NSLOT; s++) {
                     const float2 X = v[slot_c(s)];
                     v[slot_c(s)] = diff_one<EXACT>(X, prev[s]);
+                    if (CLOCK && rot) v[slot_c(s)] = dabb_clock::cmul(v[slot_c(s)], clk_phasor(s));
                     prev[s] = X;
                     if (sidx[s] < SB_DUMMY) level_acc(ls, level_l1(v[slot_c(s)]));
                 }
@@ -547,7 +571,11 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
             for (int s = 0; s < NSLOT; s++) {
                 const float2 X = v[slot_c(s)];
                 int8_t sre, sim; float2 r1;
-                demap_one<EXACT>(X, prev[s], sre, sim, r1);
+                if (CLOCK) {
+                    r1 = diff_one<EXACT>(X, prev[s]);
+                    if (rot) r1 = dabb_clock::cmul(r1, clk_phasor(s));
+                    demap_r1(r1, sre, sim);
+                } else demap_one<EXACT>(X, prev[s], sre, sim, r1);
                 sbuf[sidx[s]] = (uint16_t)((uint8_t)sre | ((uint16_t)(uint8_t)sim << 8));
                 if (TAP) { const int c0 = tb.invperm[t + 128 * slot_c(s)]; if (c0 >= 0) p.r1[((int64_t)f * 75 + (l - 1)) * KC + c0] = r1; }
                 prev[s] = X;
@@ -1105,13 +1133,15 @@ void launch_ofdm_demod(const DevTables& tb, const OfdmParams& p_in, int fft_mode
     const size_t sm = sizeof(DemodSmem);
     const dim3 grid(p.n_full * p.groups + (p.n_frames - p.n_full) * p.tail_groups), block(OFDM_THREADS);
     const bool tap = p.r1 != nullptr, fast = p.nco_fast != 0 && p.nco != nullptr;
-#define LAUNCH(E, T, F, W) do { set_smem(ofdm_demod_kernel<E, T, F, W>, sm); ofdm_demod_kernel<E, T, F, W><<<grid, block, sm, st>>>(tb, p); } while (0)
-#define LAUNCH_W(E, T, F) do { if (p.weighted) LAUNCH(E, T, F, true); else LAUNCH(E, T, F, false); } while (0)
+#define LAUNCH(E, T, F, W, C) do { set_smem(ofdm_demod_kernel<E, T, F, W, C>, sm); ofdm_demod_kernel<E, T, F, W, C><<<grid, block, sm, st>>>(tb, p); } while (0)
+#define LAUNCH_C(E, T, F, W) do { if (p.clock) LAUNCH(E, T, F, W, true); else LAUNCH(E, T, F, W, false); } while (0)
+#define LAUNCH_W(E, T, F) do { if (p.weighted) LAUNCH_C(E, T, F, true); else LAUNCH_C(E, T, F, false); } while (0)
 #define LAUNCH_F(E, T) do { if (fast) LAUNCH_W(E, T, true); else LAUNCH_W(E, T, false); } while (0)
     if (fft_mode == 0) { if (tap) LAUNCH_F(true, true); else LAUNCH_F(true, false); }
     else { if (tap) LAUNCH_F(false, true); else LAUNCH_F(false, false); }
 #undef LAUNCH_F
 #undef LAUNCH_W
+#undef LAUNCH_C
 #undef LAUNCH
 }
 
@@ -1123,8 +1153,8 @@ int ofdm_tail_frames(int n_frames)
     if (!resident) {
         int dev = 0, sms = 0, per_sm = 0;
         cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        set_smem(ofdm_demod_kernel<true, false, false, false>, sizeof(DemodSmem));
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ofdm_demod_kernel<true, false, false, false>, OFDM_THREADS, sizeof(DemodSmem));
+        set_smem(ofdm_demod_kernel<true, false, false, false, false>, sizeof(DemodSmem));
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ofdm_demod_kernel<true, false, false, false, false>, OFDM_THREADS, sizeof(DemodSmem));
         resident = sms * (per_sm > 0 ? per_sm : 1);
     }
     if (n_frames < 2 * resident) return 0;

@@ -19,6 +19,7 @@ MAX_SUBCH = 4
 FFT_EXACT, FFT_FMA = 0, 1
 NCO_EXACT, NCO_FAST = 0, 1
 DEMAP_REFERENCE, DEMAP_WEIGHTED = 0, 1
+CLOCK_OFF, CLOCK_TRACK = 0, 1
 IQ_CF32, IQ_U8, IQ_S8, IQ_S16LE, IQ_S16BE = 0, 1, 2, 3, 4
 FRAME_DECODED, FRAME_NEED_SAMPLES, FRAME_NO_SYNC, FRAME_ACQUIRING = 0, 1, 2, 3
 
@@ -38,6 +39,8 @@ class Options(C.Structure):
     _fields_ = [("disable_coarse", C.c_int32), ("fft_placement", C.c_int32), ("freqsync_method", C.c_int32), ("decode_tii", C.c_int32), ("count_bit_errors", C.c_int32), ("reserved", C.c_int32 * 3)]
     # dabb_options.soft_demap is the C struct's former reserved[0]: the ctypes layout keeps the word inside `reserved`
     soft_demap = property(lambda self: self.reserved[0], lambda self, v: self.reserved.__setitem__(0, v))
+    # dabb_options.sample_clock, the former reserved[1]
+    sample_clock = property(lambda self: self.reserved[1], lambda self, v: self.reserved.__setitem__(1, v))
 
 
 PLACEMENT_THRESHOLD_BEFORE_PEAK, PLACEMENT_STRONGEST_PEAK, PLACEMENT_EARLIEST_PEAK_WITH_BINNING = 0, 1, 2
@@ -75,6 +78,9 @@ assert TII_DTYPE.itemsize == 16 + 16 * TII_MAX
 BER_DTYPE = np.dtype([("fic_bits", "<i4"), ("fic_errors", "<i4"), ("fic_erasures", "<i4"), ("reserved", "<i4"),
                       ("subch", [("codewords", "<i4"), ("bits", "<i4"), ("errors", "<i4"), ("erasures", "<i4")], (MAX_SUBCH,))])
 assert BER_DTYPE.itemsize == 80
+# dabb_clock_result: one stream's sample-clock estimate of one step (tap 11)
+CLOCK_DTYPE = np.dtype([("ppm", "<f4"), ("applied_ppm", "<f4"), ("frames", "<i4"), ("reserved", "<i4")])
+assert CLOCK_DTYPE.itemsize == 16
 
 
 class IO(C.Structure):
@@ -85,7 +91,7 @@ class IO(C.Structure):
 
 EXPORTS = ["dabb_create", "dabb_destroy", "dabb_last_error", "dabb_abi_version", "dabb_stream_reset", "dabb_set_options", "dabb_get_info", "dabb_select_subchannel",
            "dabb_remove_subchannel", "dabb_process", "dabb_process_async", "dabb_sync", "dabb_join_lanes", "dabb_submit", "dabb_collect", "dabb_cuda_stream", "dabb_kernel_launches",
-           "dabb_read_tap", "dabb_profile", "dabb_profile_read", "dabb_ofdm_demod", "dabb_find_index", "dabb_find_index_ex", "dabb_coarse_estimate", "dabb_viterbi", "dabb_fic_decode", "dabb_msc_decode",
+           "dabb_read_tap", "dabb_profile", "dabb_profile_read", "dabb_ofdm_demod", "dabb_ofdm_demod_ex", "dabb_find_index", "dabb_find_index_ex", "dabb_coarse_estimate", "dabb_viterbi", "dabb_fic_decode", "dabb_msc_decode",
            "dabb_rs_superframes", "dabb_dev_alloc", "dabb_dev_free", "dabb_memcpy_h2d", "dabb_memcpy_d2h",
            "dabb_chan_create", "dabb_chan_destroy", "dabb_chan_input_range", "dabb_channelize", "dabb_survey", "dabb_survey_candidates"]
 
@@ -353,18 +359,20 @@ class Context:
         self._ck(self.lib.dabb_get_info(self.h, int(what), C.byref(v)))
         return v.value
 
-    def set_options(self, disable_coarse=True, fft_placement=0, freqsync_method=0, decode_tii=False, count_bit_errors=False, soft_demap=DEMAP_REFERENCE):
+    def set_options(self, disable_coarse=True, fft_placement=0, freqsync_method=0, decode_tii=False, count_bit_errors=False, soft_demap=DEMAP_REFERENCE,
+                    sample_clock=CLOCK_OFF):
         """soft_demap: DEMAP_REFERENCE (the reference's demap) or DEMAP_WEIGHTED (weak carriers scaled by their level over the symbol's
-        geometric-mean level, see dabb_options.soft_demap)"""
+        geometric-mean level, see dabb_options.soft_demap); sample_clock: CLOCK_OFF or CLOCK_TRACK (each stream's sample-clock error
+        estimated from its frame timing and its phase ramp removed from the softbits, see dabb_options.sample_clock)"""
         o = Options(); o.disable_coarse, o.fft_placement, o.freqsync_method, o.decode_tii = int(disable_coarse), int(fft_placement), int(freqsync_method), int(decode_tii)
-        o.count_bit_errors, o.soft_demap = int(count_bit_errors), int(soft_demap)
+        o.count_bit_errors, o.soft_demap, o.sample_clock = int(count_bit_errors), int(soft_demap), int(sample_clock)
         self._ck(self.lib.dabb_set_options(self.h, C.byref(o)))
 
     def read_tap(self, what, stride=0):
         """0 softbits, 1 CIR, 2 constellation points (75 x 16 per stream), 3 null symbol (2656 samples, NCO applied),
         4 TII spectra (PRS, null symbol), 5 frame results, 6 FIBs, 7 logical frames [S, MAX_SUBCH, 4, stride] and 8 superframes
         [S, MAX_SUBCH, stride] of the last step (also after process_async), 9 TII measurements (TII_DTYPE per stream), 10 channel bit
-        errors (BER_DTYPE per stream)"""
+        errors (BER_DTYPE per stream), 11 sample-clock estimates (CLOCK_DTYPE per stream)"""
         if what == 7:
             out = np.zeros((self.n_streams, MAX_SUBCH, 4, stride), np.uint8)
         elif what == 8:
@@ -385,6 +393,8 @@ class Context:
             out = np.zeros(self.n_streams, TII_DTYPE)
         elif what == 10:
             out = np.zeros(self.n_streams, BER_DTYPE)
+        elif what == 11:
+            out = np.zeros(self.n_streams, CLOCK_DTYPE)
         else:
             out = np.zeros((self.n_streams, TU), np.float32)
         self._ck(self.lib.dabb_read_tap(self.h, what, _vp(out), C.c_size_t(out.nbytes)))
@@ -412,24 +422,29 @@ class Context:
         return psd
 
     # ---- stage-level (numpy in / numpy out; device staging through the ABI)
-    def ofdm_demod(self, iq_frames, prs_start, nco=None, want_r1=False, want_fc=False):
-        """iq_frames: [n, stride] complex64; prs_start: [n] sample offsets of the first useful PRS sample"""
+    def ofdm_demod(self, iq_frames, prs_start, nco=None, want_r1=False, want_fc=False, clock_ppm=None):
+        """iq_frames: [n, stride] complex64; prs_start: [n] sample offsets of the first useful PRS sample; clock_ppm: None
+        (dabb_ofdm_demod) or [n] float32 sample-clock ppm whose phase ramp each frame's demap removes (dabb_ofdm_demod_ex)"""
         iq = np.ascontiguousarray(iq_frames, np.complex64); n, stride = iq.shape
         d_iq = self.dev(iq); d_ps = self.dev(np.ascontiguousarray(prs_start, np.int64))
         d_soft = self.dev(n * SOFT_PER_FRAME)
         d_r1 = self.dev(n * 75 * K * 8) if want_r1 else None
         d_fc = self.dev(n * 8) if want_fc else None
         d_nco = self.dev(np.ascontiguousarray(nco, np.int32)) if nco is not None else None
-        self._ck(self.lib.dabb_ofdm_demod(self.h, C.c_void_p(d_iq.ptr), C.c_int64(stride), C.c_void_p(d_ps.ptr), n,
-                                          C.c_void_p(d_nco.ptr) if d_nco else None, C.c_void_p(d_soft.ptr),
-                                          C.c_void_p(d_r1.ptr) if d_r1 else None, C.c_void_p(d_fc.ptr) if d_fc else None))
+        d_clk = self.dev(np.ascontiguousarray(clock_ppm, np.float32)) if clock_ppm is not None else None
+        head = (self.h, C.c_void_p(d_iq.ptr), C.c_int64(stride), C.c_void_p(d_ps.ptr), n, C.c_void_p(d_nco.ptr) if d_nco else None)
+        tail = (C.c_void_p(d_soft.ptr), C.c_void_p(d_r1.ptr) if d_r1 else None, C.c_void_p(d_fc.ptr) if d_fc else None)
+        if d_clk is None:
+            self._ck(self.lib.dabb_ofdm_demod(*head, *tail))
+        else:
+            self._ck(self.lib.dabb_ofdm_demod_ex(*head, C.c_void_p(d_clk.ptr), *tail))
         self.sync()
         out = [d_soft.download(np.int8).reshape(n, 75, 3072)]
         if want_r1:
             out.append(d_r1.download(np.complex64).reshape(n, 75, K))
         if want_fc:
             out.append(d_fc.download(np.complex64))
-        for b in (d_iq, d_ps, d_soft, d_r1, d_fc, d_nco):
+        for b in (d_iq, d_ps, d_soft, d_r1, d_fc, d_nco, d_clk):
             if b:
                 b.free()
         return out[0] if len(out) == 1 else tuple(out)

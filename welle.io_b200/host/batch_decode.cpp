@@ -2,7 +2,7 @@
  * batch_decode.cpp — native batch driver over the C ABI: decodes many RAW IQ recordings at once, one stream per file (or per ensemble of a
  * wideband file, --rate), on one GPU.
  *
- *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference]
+ *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock]
  *                [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file1 [file2 ...]
  *
  * What `welle-cli -f FILE -D` does for one recording (welle-cli.cpp:215-235,612-707: dump the FIC, tune to the first audio
@@ -24,9 +24,14 @@
  * leaves the options untouched; weighted scales down the softbits of carriers below the symbol's geometric-mean level, which helps the
  * Viterbi decoder in multipath (DABB_DEMAP_WEIGHTED).
  *
+ * --clock: sample-clock tracking (dabb_options.sample_clock = DABB_CLOCK_TRACK) in every context the driver creates, the --scan /
+ * --offset auto survey and confirmation contexts included: each stream estimates its recording's sample-clock error from its frame
+ * timing and the demodulator removes the phase ramp it puts on the softbits.  Every decoded frame adds one line "ppm applied_ppm frames"
+ * (tap 11) to DIR/<name>.clk.
+ *
  * --rate HZ --offset HZ[,HZ...]: every file is a wideband recording at HZ samples/s (any rate dabb_chan_create accepts) and every offset
  * (Hz from the tuned frequency, may be negative) is one stream of the batch, decoded by a channelizer of the same context (dabb_chan_*):
- * outputs go to DIR/<name>@<offset>.{fic,msc,rs} (and .tii / .ber), in the formats above.  The streams of one file progress
+ * outputs go to DIR/<name>@<offset>.{fic,msc,rs} (and .tii / .ber / .clk), in the formats above.  The streams of one file progress
  * independently (their own position, acquisition and end of file).  Every step channelizes exactly each stream's [pos, pos + need) of its
  * 2.048 Msps axis into that stream's device window and then runs dabb_process on the windows; the channelizer keeps no state, so nothing
  * is shifted on the device, and the host keeps per file only the input span its live streams still need.
@@ -69,7 +74,7 @@
 namespace {
 
 struct Stream {
-    std::string path, name; FILE* in = nullptr; FILE* fic = nullptr; FILE* msc = nullptr; FILE* rs = nullptr; FILE* tii = nullptr; FILE* ber = nullptr;
+    std::string path, name; FILE* in = nullptr; FILE* fic = nullptr; FILE* msc = nullptr; FILE* rs = nullptr; FILE* tii = nullptr; FILE* ber = nullptr; FILE* clk = nullptr;
     int64_t buf_start = 0, have = 0, pos = 0, acq_need = 0;      /* logical sample indices; `have` samples are buffered from buf_start */
     bool tracking = false, eof = false, done = false;
     std::unique_ptr<dabb_host::FigDb> db{new dabb_host::FigDb()};
@@ -90,6 +95,7 @@ struct Wide {
 
 struct Outputs {
     std::vector<dabb_frame_result> res; std::vector<uint8_t> fibs, msc, sf; std::vector<dabb_tii_result> tres; std::vector<dabb_ber_result> bres;
+    std::vector<dabb_clock_result> cres;        /* tap 11, read after every step when not empty (--clock) */
 };
 
 /* the receiver position after one step's result r of stream s: 0 = the stream ended, 1 = no frame decoded, 2 = a frame was decoded */
@@ -122,6 +128,10 @@ bool handle_result(dabb_ctx* ctx, Stream& z, int s, const Outputs& o, bool tii, 
     if (ber) {
         const dabb_ber_result& b = o.bres[(size_t)s];
         fprintf(z.ber, "%d %d %d %d %d %d %d\n", b.fic_bits, b.fic_errors, b.fic_erasures, b.subch[0].codewords, b.subch[0].bits, b.subch[0].errors, b.subch[0].erasures);
+    }
+    if (z.clk) {
+        const dabb_clock_result& c = o.cres[(size_t)s];
+        fprintf(z.clk, "%.4f %.4f %d\n", c.ppm, c.applied_ppm, c.frames);
     }
     for (int f = 0; f < 12; f++) {
         const uint8_t* fb = o.fibs.data() + ((size_t)s * 12 + (size_t)f) * 32;
@@ -194,6 +204,7 @@ bool step(dabb_ctx* ctx, Outputs& o, std::vector<int64_t>& buf_start, const floa
     if (dabb_process(ctx, &io) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     if (tii && dabb_read_tap(ctx, 9, o.tres.data(), o.tres.size() * sizeof(dabb_tii_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     if (ber && dabb_read_tap(ctx, 10, o.bres.data(), o.bres.size() * sizeof(dabb_ber_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
+    if (!o.cres.empty() && dabb_read_tap(ctx, 11, o.cres.data(), o.cres.size() * sizeof(dabb_clock_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     return true;
 }
 
@@ -310,13 +321,15 @@ bool run_wide(dabb_ctx* ctx, std::vector<Stream>& st, std::vector<Wide>& wf, int
 
 std::string base_name(const std::string& path) { const size_t slash = path.find_last_of('/'); return slash == std::string::npos ? path : path.substr(slash + 1); }
 
-/* a context of the scan with dabb_options.soft_demap = soft (--soft); the other options as cfg gives them; false on an error */
-static bool create_scan_ctx(const dabb_config& cfg, int soft, dabb_ctx** ctx)
+/* a context of the scan with dabb_options.soft_demap = soft (--soft) and sample_clock = clock (--clock); the other options as cfg gives
+ * them; false on an error */
+static bool create_scan_ctx(const dabb_config& cfg, int soft, int clock, dabb_ctx** ctx)
 {
     if (dabb_create(&cfg, ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return false; }
-    if (soft == DABB_DEMAP_REFERENCE) return true;
+    if (soft == DABB_DEMAP_REFERENCE && clock == DABB_CLOCK_OFF) return true;
     dabb_options op; memset(&op, 0, sizeof op);
     op.disable_coarse = cfg.disable_coarse; op.fft_placement = cfg.fft_placement; op.freqsync_method = cfg.freqsync_method; op.soft_demap = soft;
+    op.sample_clock = clock;
     if (dabb_set_options(*ctx, &op) == DABB_OK) return true;
     fprintf(stderr, "batch_decode: %s\n", dabb_last_error(*ctx));
     dabb_destroy(*ctx);
@@ -325,7 +338,7 @@ static bool create_scan_ctx(const dabb_config& cfg, int soft, dabb_ctx** ctx)
 }
 
 /* --scan: the ensembles of every file (ascending offset, per file), as the streams of their confirmation decode; false on an error */
-bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int device, int soft, std::vector<std::vector<Stream>>& found)
+bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int device, int soft, int clock, std::vector<std::vector<Stream>>& found)
 {
     const int64_t TF = DABB_TF;
     const int bps = bytes_per_sample(fmt);
@@ -357,7 +370,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
     dabb_config cfg; memset(&cfg, 0, sizeof cfg);
     cfg.abi_version = DABB_ABI_VERSION; cfg.device = device; cfg.n_streams = 1; cfg.transmission_mode = 1;
     dabb_ctx* ctx = nullptr;
-    if (!create_scan_ctx(cfg, soft, &ctx)) return false;
+    if (!create_scan_ctx(cfg, soft, clock, &ctx)) return false;
     std::vector<float> psd(files.size() * (size_t)nfft);
     dabb_survey_io sio; memset(&sio, 0, sizeof sio);
     sio.in = buf.data(); sio.in_is_host = 1; sio.iq_format = fmt; sio.in_stride = in_len; sio.n_inputs = (int32_t)files.size(); sio.nfft = nfft;
@@ -390,7 +403,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
         const int S = (int)cs.size();
         if (S == 0) return true;
         cfg.n_streams = S; cfg.disable_coarse = disable_coarse; cfg.freqsync_method = freqsync;
-        if (!create_scan_ctx(cfg, soft, &ctx)) return false;
+        if (!create_scan_ctx(cfg, soft, clock, &ctx)) return false;
         dabb_stream_reset(ctx, 0, S, 0);
         Outputs o; o.res.resize((size_t)S); o.fibs.resize((size_t)S * 12 * 32);
         std::vector<int64_t> buf_start((size_t)S);
@@ -459,7 +472,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
 
 int main(int argc, char** argv)
 {
-    int fmt = DABB_IQ_CF32, device = 0, soft = DABB_DEMAP_REFERENCE; bool coarse = false, tii = false, ber = false; std::string out;
+    int fmt = DABB_IQ_CF32, device = 0, soft = DABB_DEMAP_REFERENCE, clock = DABB_CLOCK_OFF; bool coarse = false, tii = false, ber = false; std::string out;
     int64_t rate = 0; std::vector<int64_t> offsets; bool scan_only = false, auto_offsets = false;
     std::vector<std::string> files;
     for (int i = 1; i < argc; i++) {
@@ -474,6 +487,7 @@ int main(int argc, char** argv)
         else if (a == "--coarse") coarse = true;
         else if (a == "--tii") tii = true;
         else if (a == "--ber") ber = true;
+        else if (a == "--clock") clock = DABB_CLOCK_TRACK;
         else if (a == "--soft" && i + 1 < argc) {
             const std::string m = argv[++i];
             soft = m == "reference" ? DABB_DEMAP_REFERENCE : m == "weighted" ? DABB_DEMAP_WEIGHTED : -1;
@@ -494,7 +508,7 @@ int main(int argc, char** argv)
     }
     if (out.empty() || files.empty() || (rate > 0) != ((int)!offsets.empty() + (int)scan_only + (int)auto_offsets == 1)
         || (rate <= 0 && (scan_only || auto_offsets))) {
-        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
+        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
         return 2;
     }
     const bool wide = rate > 0;
@@ -502,7 +516,7 @@ int main(int argc, char** argv)
     std::vector<std::vector<int64_t>> file_offsets(wide ? files.size() : 0, offsets);
     if (scan_only || auto_offsets) {
         std::vector<std::vector<Stream>> found;
-        if (!scan(files, rate, fmt, device, soft, found)) return 1;
+        if (!scan(files, rate, fmt, device, soft, clock, found)) return 1;
         for (size_t f = 0; f < files.size(); f++) {
             file_offsets[f].clear();
             for (const Stream& z : found[f]) file_offsets[f].push_back(z.offset + z.corr);
@@ -536,9 +550,9 @@ int main(int argc, char** argv)
     cfg.disable_coarse = coarse ? 0 : 1; cfg.n_subch_slots = DABB_MAX_SUBCH; cfg.max_subch_cu = 416;
     dabb_ctx* ctx = nullptr;
     if (dabb_create(&cfg, &ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return 1; }
-    if (tii || ber || soft != DABB_DEMAP_REFERENCE) {
+    if (tii || ber || soft != DABB_DEMAP_REFERENCE || clock != DABB_CLOCK_OFF) {
         dabb_options op; memset(&op, 0, sizeof op);
-        op.disable_coarse = cfg.disable_coarse; op.decode_tii = tii; op.count_bit_errors = ber; op.soft_demap = soft;
+        op.disable_coarse = cfg.disable_coarse; op.decode_tii = tii; op.count_bit_errors = ber; op.soft_demap = soft; op.sample_clock = clock;
         if (dabb_set_options(ctx, &op) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
     }
 
@@ -561,14 +575,15 @@ int main(int argc, char** argv)
         z.fic = fopen((out + "/" + z.name + ".fic").c_str(), "wb"); z.msc = fopen((out + "/" + z.name + ".msc").c_str(), "wb"); z.rs = fopen((out + "/" + z.name + ".rs").c_str(), "w");
         if (tii) z.tii = fopen((out + "/" + z.name + ".tii").c_str(), "w");
         if (ber) z.ber = fopen((out + "/" + z.name + ".ber").c_str(), "w");
-        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii) || (ber && !z.ber)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
+        if (clock) z.clk = fopen((out + "/" + z.name + ".clk").c_str(), "w");
+        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii) || (ber && !z.ber) || (clock && !z.clk)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
         z.acq_need = 3 * TF;
     }
     dabb_stream_reset(ctx, 0, S, 0);
 
     Outputs o;
     o.res.resize((size_t)S); o.fibs.resize((size_t)S * 12 * 32); o.msc.resize((size_t)S * DABB_MAX_SUBCH * 4 * 1152); o.sf.resize((size_t)S * DABB_MAX_SUBCH * 5760);
-    o.tres.resize(tii ? (size_t)S : 0); o.bres.resize(ber ? (size_t)S : 0);
+    o.tres.resize(tii ? (size_t)S : 0); o.bres.resize(ber ? (size_t)S : 0); o.cres.resize(clock ? (size_t)S : 0);
     std::vector<int64_t> buf_start((size_t)S);
 
     int active = S;
@@ -626,7 +641,7 @@ int main(int argc, char** argv)
     for (auto& z : st) {
         printf("%s frames=%ld fibs=%ld fib_crc_ok=%ld service=0x%X bitrate=%d logical_frames=%ld\n", z.name.c_str(), z.frames, z.fibs, z.fibs_ok, z.sid, z.bitrate, z.logical);
         if (z.in) fclose(z.in);
-        fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii); if (z.ber) fclose(z.ber);
+        fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii); if (z.ber) fclose(z.ber); if (z.clk) fclose(z.clk);
     }
     dabb_destroy(ctx);
     return 0;
