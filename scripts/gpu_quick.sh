@@ -1,5 +1,5 @@
 #!/bin/bash
-# quick GPU check: all parity tests, then the short headline bench (per-kernel times) of the default library and of every variant_*.so
+# quick GPU check: all parity tests, then the short headline bench (per-kernel times) of the default library
 mkdir -p gpurun_out
 if [ -z "${SKIP_TESTS:-}" ]; then python -m pytest tests -m gpu -q -x 2>&1 | tail -8 > gpurun_out/pytest_quick.log; tail -3 gpurun_out/pytest_quick.log; fi
 one() {
@@ -17,4 +17,3 @@ PY
 }
 unset DABB_LIB
 one default
-for lib in $(ls variant_*.so 2>/dev/null); do export DABB_LIB=$PWD/$lib; one "$lib"; done

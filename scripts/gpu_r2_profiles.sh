@@ -1,9 +1,8 @@
 #!/bin/bash
-# one GPU call: Viterbi thread-mapping microbenchmark + the round's ncu captures (launch list, full sets of the OFDM kernel with the
-# oscillator off / fast / exact, and of the MSC Viterbi launch)
+# one GPU call: the round's ncu captures (launch list, full sets of the OFDM kernel with the oscillator off / fast / exact, and of the
+# MSC Viterbi launch)
 set -u
 mkdir -p gpurun_out
-if [ -x ./gpurun_exp_vit_threads ]; then timeout 120 ./gpurun_exp_vit_threads > gpurun_out/ubench_vit_threads.txt 2>&1; fi
 
 bash scripts/gpu_ncu.sh 8192
 BENCH="python bench.py --batch 8192 --steps 3 --warmup 8 --no-cpu-baseline --no-e2e --no-other-configs"

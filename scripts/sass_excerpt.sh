@@ -7,7 +7,7 @@ out=${1:-profiles/sass_excerpts.txt}        # profiles/ is git-ignored: a local 
 mkdir -p "$(dirname "$out")"
 {
 echo "# cuobjdump -sass of welle.io_b200/csrc/build/{ofdm,viterbi}.o (sm_90a), $(date -u +%Y-%m-%d)"
-for spec in "ofdm.o|ofdm_demod_kernelILb1ELb0ELb0|UBLKCP SYNCS FMUL FADD MUFU F2I STS.U16 LDS.128" "ofdm.o|find_index_kernelILb1ELb1|FMUL FADD DSETP DFMA" "viterbi.o|viterbi_kernelILb0|VIMNMX PRMT LDGSTS IDP IMAD.IADD IADD3 STG.E.64 CCTL" "rs.o|superframe_kernel|LDS STS"; do
+for spec in "ofdm.o|ofdm_demod_kernelILb1ELb0ELb0|UBLKCP SYNCS FMUL FADD MUFU F2I STS.U16 LDS.128" "ofdm.o|find_index_kernelILb1EE|FMUL FADD DSETP DFMA" "viterbi.o|viterbi_kernelILb0|VIMNMX PRMT LDGSTS IDP IMAD.IADD IADD3 STG.E.64 CCTL" "rs.o|superframe_kernel|LDS STS"; do
     obj=${spec%%|*}; rest=${spec#*|}; pat=${rest%%|*}; mn=${rest#*|}
     sass=$(cuobjdump -sass welle.io_b200/csrc/build/$obj | awk -v p="$pat" '$0 ~ "Function : " {f = ($0 ~ p)} f')
     [ -z "$sass" ] && continue

@@ -1,5 +1,5 @@
-"""The Viterbi and Reed-Solomon decoders at their arithmetic limits, on the CPU: the per-thread code of the kernels (viterbi_core.cuh,
-viterbi_core2.cuh compiled as plain C++, tests/host_emul) and the oracle against the plain wide-integer references of
+"""The Viterbi and Reed-Solomon decoders at their arithmetic limits, on the CPU: the per-thread code of the kernels (viterbi_core.cuh
+compiled as plain C++, tests/host_emul) and the oracle against the plain wide-integer references of
 tests/plainref.py, on inputs chosen to break a packed 16-bit decoder (ties, pinned symbols, the largest metric spread, patterns aligned
 with the register layouts and the 24-step stage) instead of random ones; and the superframe builder, the RS syndrome check and the
 oracle's superframe handling for all four DAB+ audio formats, with the unmodified reference's stored answers
@@ -24,7 +24,7 @@ NBITS = (192, 768, 2304, 9216)           # 9216 = 24 x 384, the longest MSC code
 def emul(tmp_path_factory):
     d = tmp_path_factory.mktemp("emul")
     libs = {}
-    for name in ("emul_viterbi", "emul_vitdec", "emul_viterbi2"):
+    for name in ("emul_viterbi", "emul_vitdec"):
         so = str(d / f"lib{name}.so")
         subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", so, os.path.join(HERE, "host_emul", name + ".cpp")])
         libs[name] = C.CDLL(so)
@@ -81,15 +81,15 @@ def test_profiles_exist(oracle):
     assert [p[0] for p in _profiles(oracle)] == ["fic", "a8/1", "a96/3", "a192/4", "a384/1", "b32/1", "b192/4", "u32/5", "u192/2", "u384/5"]
 
 
-@pytest.mark.parametrize("variant", ["one_thread", "two_threads"])
+@pytest.mark.parametrize("variant", ["one_thread"])
 def test_decoder_emulation_families_as_fragments(emul, oracle, variant):
-    """one thread (pair of threads) of the decoder kernel - expansion tables, 8-byte window, packed ACS, 24-step traceback, de-dispersal,
+    """one thread of the decoder kernel - expansion tables, 8-byte window, packed ACS, 24-step traceback, de-dispersal,
     packing - on the families as PUNCTURED fragments: output bytes == pack(dedisperse(viterbi_plain(depuncture(fragment)))).  The
     fragment starts on a 16-byte boundary, ends on one, or ends one byte behind one; random bytes follow it.  (-128 is not an input of
     this code: the stage entry points map it to -127 first, which tests/test_gpu_decoder_limits.py covers.)  The de-puncturing map is the
     one the library builds for the profile (tables.cpp), and must mark exactly the softbits the puncturing vectors transmit - also for
     EEP 1-A at 384 kbit/s, whose 36 864 softbits per codeword do not fit a 16-bit index."""
-    fn = emul["emul_vitdec"].emul_vitdec if variant == "one_thread" else emul["emul_viterbi2"].emul_vitdec2
+    fn = emul["emul_vitdec"].emul_vitdec
     rng = np.random.default_rng(31)
     for pname, blocks, nbits, args in _profiles(oracle):
         mask = P.puncture_mask(blocks); n_in = int(mask.sum())

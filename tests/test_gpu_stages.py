@@ -93,10 +93,9 @@ def test_find_index(ctx, oracle, iq12):
 def test_find_index_threshold_search_many_windows(oracle, iq12):
     """ThresholdBeforePeak over the whole range of peak positions (window starts swept over more than a symbol, so the correlation peak
     lands everywhere incl. the first 200 and the last samples, and outside: no synchronisation), on clean, noisy, pre-echo and
-    noise-only input.  The library's warp-per-window search (no sliding maximum: DESIGN.md 3) and its literal sliding-maximum form
-    (DABB_SEARCH_GENERIC) must both equal the oracle's index for every window."""
+    noise-only input.  The library's warp-per-window search (no sliding maximum: DESIGN.md 3) must equal the oracle's index for every
+    window."""
     from conftest import load_pkg
-    import os
     pkg = load_pkg()
     tx, iq = iq12
     rng = np.random.default_rng(77)
@@ -111,17 +110,11 @@ def test_find_index_threshold_search_many_windows(oracle, iq12):
     frames = np.stack(frames); starts = np.zeros(len(frames), np.int64)
     exp = np.array([oracle.find_index(frames[i])[0] for i in range(len(frames))])
     assert len(set(exp.tolist())) > 100 and (exp < 0).any() and (exp < 200).any() and (exp > 1800).any()
-    for generic in (False, True):
-        if generic:
-            os.environ["DABB_SEARCH_GENERIC"] = "1"
-        try:
-            c = pkg.Context(n_streams=len(starts))
-        finally:
-            os.environ.pop("DABB_SEARCH_GENERIC", None)
-        idx = c.find_index(frames, starts)
-        c.close()
-        bad = np.nonzero(idx != exp)[0]
-        assert bad.size == 0, (generic, bad[:10], idx[bad[:10]], exp[bad[:10]])
+    c = pkg.Context(n_streams=len(starts))
+    idx = c.find_index(frames, starts)
+    c.close()
+    bad = np.nonzero(idx != exp)[0]
+    assert bad.size == 0, (bad[:10], idx[bad[:10]], exp[bad[:10]])
 
 
 @pytest.mark.parametrize("placement", [1, 2])

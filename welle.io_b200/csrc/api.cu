@@ -107,7 +107,7 @@ struct dabb_ctx {
     DevBuf<float2> d_tw_fwd, d_tw_inv, d_prs_ref, d_osc; DevBuf<int16_t> d_invperm, d_fic_map; DevBuf<uint8_t> d_gf_exp, d_gf_log; DevBuf<double2> d_osc_hi;   // what `dev` points into
     DevBuf<StreamState> d_state; DevBuf<StepScratch> d_scr; DevBuf<MscSlotState> d_slots;
     DevBuf<int64_t> d_buf_start, d_win, d_prs; DevBuf<int32_t> d_nco_sync, d_nco_frame;
-    DevBuf<int32_t> d_active, d_index; DevBuf<float> d_cir, d_cir_work; int search_generic = 0; DevBuf<float2> d_r1, d_null; DevBuf<int32_t> d_snr; DevBuf<float2> d_fc; DevBuf<float> d_lvl;
+    DevBuf<int32_t> d_active, d_index; DevBuf<float> d_cir, d_cir_work; DevBuf<float2> d_r1, d_null; DevBuf<int32_t> d_snr; DevBuf<float2> d_fc; DevBuf<float> d_lvl;
     DevBuf<int8_t> d_soft; DevBuf<uint2> d_fic_steptab; DevBuf<uint32_t> d_fic_stage_off; DevBuf<uint2> d_dec; DevBuf<uint8_t> d_fibs; DevBuf<int32_t> d_crc;
     DevBuf<dabb_frame_result> d_results;
     // the protection-profile table: one entry per distinct ProtProfile a select call has met, built the first time it is selected and
@@ -766,7 +766,6 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
         cudaMemcpy(ctx->d_fic_steptab, steps.data(), steps.size() * sizeof(uint2), cudaMemcpyHostToDevice);
         cudaMemcpy(ctx->d_fic_stage_off, soff.data(), soff.size() * 4, cudaMemcpyHostToDevice);
     }
-    ctx->search_generic = getenv("DABB_SEARCH_GENERIC") != nullptr;     // A/B: ThresholdBeforePeak through the literal sliding maximum
     if (getenv("DABB_TRACE")) {
         ctx->trace_path = getenv("DABB_TRACE"); ctx->trace.cap = 1u << 20;
         if ((rc = dalloc(ctx, ctx->d_trace_rec, (size_t)3 * ctx->trace.cap)) || (rc = dalloc(ctx, ctx->d_trace_count, 1))) return fail(rc);
@@ -996,13 +995,13 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     if ((rc = check_launch(ctx, "plan_kernel"))) return rc;
     SyncParams sp{}; sp.iq = iq; sp.stride = stride; sp.win_start = d_win; sp.nco = d_nco_sync; sp.active = d_active; sp.index_out = d_index; sp.cir_out = ctx->d_cir; sp.n = S;
     sp.fic_ratio = ctx->d_fic_ratio; sp.coarse_out = ctx->disable_coarse ? nullptr : ctx->d_coarse.get(); sp.placement = ctx->placement; sp.freqsync = ctx->freqsync;
-    sp.cir_work = ctx->d_cir_work; sp.search_generic = ctx->search_generic;
-    launch_find_index(ctx->dev, sp, ctx->fft_mode, A, 0);
+    sp.cir_work = ctx->d_cir_work;
+    launch_find_index(ctx->dev, sp, A, 0);
     if ((rc = check_launch(ctx, "find_index_kernel"))) return rc;
-    launch_find_index(ctx->dev, sp, ctx->fft_mode, A, 1);
+    launch_find_index(ctx->dev, sp, A, 1);
     if ((rc = check_launch(ctx, "find_search_kernel"))) return rc;
     if (sp.coarse_out) {
-        launch_find_index(ctx->dev, sp, ctx->fft_mode, A, 2);
+        launch_find_index(ctx->dev, sp, A, 2);
         if ((rc = check_launch(ctx, "find_coarse_kernel"))) return rc;
     }
     const bool track = ctx->sample_clock == DABB_CLOCK_TRACK;
@@ -1295,8 +1294,8 @@ int dabb_find_index_ex(dabb_ctx* ctx, const float* iq, int64_t stride, const int
     DevBuf<float> temp;
     int rc;
     if (n > ctx->S && (rc = dalloc(ctx, temp, (size_t)n * TU, false))) return rc;
-    sp.cir_work = temp ? temp.get() : ctx->d_cir_work.get(); sp.search_generic = ctx->search_generic;
-    launch_find_index(ctx->dev, sp, ctx->fft_mode, ctx->stream);
+    sp.cir_work = temp ? temp.get() : ctx->d_cir_work.get();
+    launch_find_index(ctx->dev, sp, ctx->stream);
     rc = check_launch(ctx, "find_index_kernel");
     if (temp) cudaStreamSynchronize(ctx->stream);
     return rc;

@@ -77,13 +77,12 @@ struct SyncParams {
     const int32_t* fic_ratio; int32_t* coarse_out;
     int placement;      // DABB_PLACEMENT_*: 0 ThresholdBeforePeak, 1 StrongestPeak, 2 EarliestPeakWithBinning
     int freqsync;       // DABB_FREQSYNC_*: 0 PatternOfZeros, 1 GetMiddle, 2 CorrelatePRS
-    int search_generic; // 1: ThresholdBeforePeak through the literal sliding-maximum search (find_search_kernel) instead of the warp-per-window form (A/B tests)
 };
 
 void launch_ofdm_demod(const DevTables& tb, const OfdmParams& p, int fft_mode, cudaStream_t st);
 int ofdm_tail_frames(int n_frames);
 constexpr int OFDM_TAIL_GROUPS = 5;              // CTAs per tail frame (15 data symbols each): the best of 5 / 15 / 25 before the port to H100
-void launch_find_index(const DevTables& tb, const SyncParams& p, int fft_mode, cudaStream_t st, int part = -1);
+void launch_find_index(const DevTables& tb, const SyncParams& p, cudaStream_t st, int part = -1);
 void launch_tii_spectra(const DevTables& tb, const float2* iq, int64_t stride, const int64_t* prs_start, const int32_t* nco_frame, const int32_t* active,
                         const float2* nulls, float2* out, int n, cudaStream_t st);
 void launch_coarse(const DevTables& tb, const float2* iq, int64_t stride, const int64_t* prs_start, int n, int freqsync, int32_t* out, cudaStream_t st);

@@ -134,8 +134,7 @@ __device__ __forceinline__ XIdx make_xidx(int t)
 // pass C: position t + 128 c -> (t ^ X(c)) + 128 c with the compile-time constant X(c) = swizzle bits of 128 c
 __device__ __forceinline__ constexpr int xc_of(int c) { return ((c & 1) << 3) | (((c >> 1) & 1) << 2) | ((c >> 2) & 3); }
 
-// FFT of the 2048 samples at src[w0 .. w0+2048) -> v[a+4b] = X[t + 128a + 512b].  Contains two __syncthreads.
-template <bool EXACT, bool INV>
+// FFT of the 2048 samples at src[w0 .. w0+2048) -> v[a+4b] = X[t + 128a + 512b], exact arithmetic.  Contains two __syncthreads.
 __device__ __forceinline__ void fft2048_from_global(const float2* __restrict__ src, int64_t w0, float2 v[16], OfdmSmem& sm, int t, const XIdx& xi,
                                                     const DevTables& tb, const Nco& nco, const float2* __restrict__ tw_c5)
 {
@@ -158,7 +157,7 @@ __device__ __forceinline__ void fft2048_from_global(const float2* __restrict__ s
 #pragma unroll
     for (int h = 0; h < 2; h++) {
         float2 y[8];
-        passA_block<EXACT, INV>(x + 8 * h, y, sm.tw);
+        passA_block<true, false>(x + 8 * h, y, sm.tw);
 #pragma unroll
         for (int e = 0; e < 8; e++) sm.xbuf[xi.a[h] ^ e] = y[e];
     }
@@ -169,7 +168,7 @@ __device__ __forceinline__ void fft2048_from_global(const float2* __restrict__ s
         for (int b = 0; b < 4; b++)
 #pragma unroll
             for (int a = 0; a < 4; a++) v[a + 4 * b] = sm.xbuf[xi.b[a] + 32 * b];
-        passB<EXACT, INV>(v, xi.kk, sm.tw);
+        passB<true, false>(v, xi.kk, sm.tw);
 #pragma unroll
         for (int b = 0; b < 4; b++)
 #pragma unroll
@@ -179,7 +178,7 @@ __device__ __forceinline__ void fft2048_from_global(const float2* __restrict__ s
     // pass C
 #pragma unroll
     for (int c = 0; c < 16; c++) v[c] = sm.xbuf[(t ^ xc_of(c)) + 128 * c];
-    passC_ldg<EXACT, INV>(v, t, tw_c5);
+    passC_ldg<true, false>(v, t, tw_c5);
 }
 
 // ---- TMA / mbarrier helpers (SASS: UBLKCP, SYNCS) ----
@@ -207,22 +206,14 @@ __device__ __forceinline__ float level_sample(float2 x) { return fabsf(x.x) + fa
 
 // (1 - 1e-5)^2552: what the reference's level tracker sLevel = 1e-5 |v|_1 + (1 - 1e-5) sLevel (ofdm-processor.cpp:166,215) forgets per symbol
 constexpr float LEVEL_DECAY_SYM = 0.97480279f;
-#ifndef DEMOD_CTAS_PER_SM
-#define DEMOD_CTAS_PER_SM 5
-#endif
 constexpr int IN_CAP = 2560;     // staged samples per symbol: 2552 + 1 (16-byte alignment shift) + 1 (round-up), padded
 constexpr int SB_DUMMY = 1536;   // softbit staging as (re, im) byte pairs indexed by logical carrier: [0,1536) real entries, then one private
                                  // dummy entry per thread for its unused bin
-// DEMOD_CTAS_PER_SM >= 6 (experiment): 37 KB of shared memory per CTA - the small twiddles come through L1 and the softbit staging
-// area lives in the exchange buffer (two more barriers per symbol) - and 80 registers
-#define DEMOD_SLIM (DEMOD_CTAS_PER_SM >= 6)
 struct __align__(16) DemodSmem {
     float2 inbuf[IN_CAP];            // 20 KB: one symbol, guard interval first, filled by one cp.async.bulk (TMA)
     float2 xbuf[TU];                 // 16 KB swizzled exchange buffer
-#if !DEMOD_SLIM
     float2 tw[TwLayout::C4];         // 1 KB: twiddles of passes A and B (pass C reads its 15 KB through L1 with __ldg)
     uint16_t sbuf[1536 + 128];        // (re | im << 8) per logical carrier: one 16-bit scatter store per carrier
-#endif
     float2 rtab[2][16];              // DABB_NCO_FAST: e^{-j theta((128 h + 256 c) Hz)} for the PRS / the data symbols
     float red[16];
     uint64_t full;                   // a transformed symbol's copy, or a light symbol's in the first half of inbuf
@@ -296,11 +287,6 @@ template <bool EXACT, bool FASTNCO>
 __device__ __forceinline__ void fft2048_from_smem(const float2* in, int64_t idx0, float2 v[16], DemodSmem& sm, int t, const XIdx& xi,
                                                   const float2* __restrict__ tw_c5, const DevTables& tb, const Nco& nco, bool afc, float2& fc, const float2* rtab, float& l1_first)
 {
-#if DEMOD_SLIM
-    const float2* twp = tb.tw_fwd;
-#else
-    const float2* twp = sm.tw;
-#endif
     // l1_first: |re| + |im| of the thread's first (mixed) sample, the sub-sampled input of the running signal level (see advance_kernel)
     if (FASTNCO && nco.mix) {
         // sample n = t + 128 h + 256 c gets osc(lp - (128 h + 256 c) Hz) = osc(lp) * rtab[8 h + c]; the guard-interval correlation is
@@ -323,7 +309,7 @@ __device__ __forceinline__ void fft2048_from_smem(const float2* in, int64_t idx0
             for (int c = 0; c < 8; c++) x[c] = cmul_fast(x[c], cmul_fast(o0, rtab[8 * h + c]));
             if (h == 0) l1_first = level_sample(x[0]);
             float2 y[8];
-            passA_block<EXACT, false>(x, y, twp);
+            passA_block<EXACT, false>(x, y, sm.tw);
 #pragma unroll
             for (int e = 0; e < 8; e++) sm.xbuf[xi.a[h] ^ e] = y[e];
         }
@@ -358,7 +344,7 @@ __device__ __forceinline__ void fft2048_from_smem(const float2* in, int64_t idx0
         }
         if (h == 0) l1_first = level_sample(x[0]);
         float2 y[8];
-        passA_block<EXACT, false>(x, y, twp);
+        passA_block<EXACT, false>(x, y, sm.tw);
 #pragma unroll
         for (int e = 0; e < 8; e++) sm.xbuf[xi.a[h] ^ e] = y[e];
     }
@@ -366,16 +352,11 @@ __device__ __forceinline__ void fft2048_from_smem(const float2* in, int64_t idx0
 template <bool EXACT>
 __device__ __forceinline__ void fft2048_finish(float2 v[16], DemodSmem& sm, int t, const XIdx& xi, const float2* __restrict__ tw_c5, const TwB2& b2)
 {
-#if DEMOD_SLIM
-    const float2* twp = tw_c5 - TwLayout::C5;
-#else
-    const float2* twp = sm.tw;
-#endif
 #pragma unroll
     for (int b = 0; b < 4; b++)
 #pragma unroll
         for (int a = 0; a < 4; a++) v[a + 4 * b] = sm.xbuf[xi.b[a] + 32 * b];
-    passB_w<EXACT, false>(v, xi.kk, twp, b2);
+    passB_w<EXACT, false>(v, xi.kk, sm.tw, b2);
 #pragma unroll
     for (int b = 0; b < 4; b++)
 #pragma unroll
@@ -384,13 +365,10 @@ __device__ __forceinline__ void fft2048_finish(float2 v[16], DemodSmem& sm, int 
 #pragma unroll
     for (int c = 0; c < 16; c++) v[c] = sm.xbuf[(t ^ xc_of(c)) + 128 * c];
     passC_ldg<EXACT, false>(v, t, tw_c5);
-#if DEMOD_SLIM
-    __syncthreads();        // the exchange buffer is about to be reused as the softbit staging area
-#endif
 }
 
 template <bool EXACT, bool TAP, bool FASTNCO, bool WEIGHTED, bool CLOCK>
-__global__ void __launch_bounds__(OFDM_THREADS, DEMOD_CTAS_PER_SM)
+__global__ void __launch_bounds__(OFDM_THREADS, 5)
 ofdm_demod_kernel(DevTables tb, OfdmParams p)
 {
     extern __shared__ __align__(16) unsigned char smraw[];
@@ -398,12 +376,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
     const int t = threadIdx.x;
     // ---- once per CTA
     if (t == 0) { mbar_init(&sm.full, 1); if (!TAP) mbar_init(&sm.half1, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-#if DEMOD_SLIM
-    uint16_t* const sbuf = reinterpret_cast<uint16_t*>(sm.xbuf);
-#else
     if (t < TwLayout::C4) sm.tw[t] = tb.tw_fwd[t];
-    uint16_t* const sbuf = sm.sbuf;
-#endif
     const float2* tw_c5 = tb.tw_fwd + TwLayout::C5;
     const XIdx xi = make_xidx(t);
     const TwB2 b2 = load_twb2(tb.tw_fwd, xi.kk);
@@ -562,7 +535,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
                     const float2 r1 = v[slot_c(s)];
                     int8_t sre, sim;
                     demap_weighted(r1, G, rG, sre, sim);
-                    sbuf[sidx[s]] = (uint16_t)((uint8_t)sre | ((uint16_t)(uint8_t)sim << 8));
+                    sm.sbuf[sidx[s]] = (uint16_t)((uint8_t)sre | ((uint16_t)(uint8_t)sim << 8));
                     if (TAP) { const int c0 = tb.invperm[t + 128 * slot_c(s)]; if (c0 >= 0) p.r1[((int64_t)f * 75 + (l - 1)) * KC + c0] = r1; }
                 }
             } else {
@@ -576,7 +549,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
                     if (rot) r1 = dabb_clock::cmul(r1, clk_phasor(s));
                     demap_r1(r1, sre, sim);
                 } else demap_one<EXACT>(X, prev[s], sre, sim, r1);
-                sbuf[sidx[s]] = (uint16_t)((uint8_t)sre | ((uint16_t)(uint8_t)sim << 8));
+                sm.sbuf[sidx[s]] = (uint16_t)((uint8_t)sre | ((uint16_t)(uint8_t)sim << 8));
                 if (TAP) { const int c0 = tb.invperm[t + 128 * slot_c(s)]; if (c0 >= 0) p.r1[((int64_t)f * 75 + (l - 1)) * KC + c0] = r1; }
                 prev[s] = X;
             }
@@ -585,7 +558,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
             // de-interleave the pairs into the reference's layout (1536 Re bits, then 1536 Im bits): thread t < 96 takes the 16-byte
             // chunks t and t + 96 of the staging area (lane-consecutive: conflict-free; 8 carriers each) and stores 8 bytes per chunk and half
             if (t < 96) {
-                const uint4* s4 = reinterpret_cast<const uint4*>(sbuf);
+                const uint4* s4 = reinterpret_cast<const uint4*>(sm.sbuf);
                 uint2* dst = reinterpret_cast<uint2*>(p.soft + (int64_t)f * p.soft_stride + (int64_t)(l - 1) * 3072);
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
@@ -599,9 +572,6 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
                     dst[192 + t + 96 * h] = im;
                 }
             }
-#if DEMOD_SLIM
-            __syncthreads();        // staging area read: the next symbol's first pass may overwrite the exchange buffer
-#endif
         } else {
             // a reference only (the PRS when l == 0, or a symbol no decoder reads before one they do): keep its spectrum, estimate SNR from the PRS
 #pragma unroll
@@ -647,9 +617,9 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// findIndex: one CTA per window.  FFT -> * conj(refTable) -> IFFT/2048 -> |.| -> 100-tap sliding maximum ->
-// threshold search.  The sum of |.| is accumulated sequentially by one thread in index order like the CPU loop
-// (phasereference.cpp:216-220) so that the `max > 3*sum/Tu` decision sees the same float.
+// findIndex: FFT -> * conj(refTable) -> IFFT/2048 -> |.| (find_index_kernel, one CTA per window), then the placement search
+// (find_search_tbp_kernel, find_search_kernel).  The sum of |.| is accumulated sequentially by one thread in index order like the
+// CPU loop (phasereference.cpp:216-220) so that the `max > 3*sum/Tu` decision sees the same float.
 // ------------------------------------------------------------------------------------------------------------
 struct __align__(16) SyncSmem {
     OfdmSmem o;
@@ -662,7 +632,6 @@ struct __align__(16) SyncSmem {
 };
 
 // coarse frequency estimate of one aligned PRS = the T_u samples at src[off ..]; collective over the CTA, result via *out
-template <bool EXACT>
 __device__ __forceinline__ void coarse_estimate(const DevTables& tb, SyncSmem& sm, const float2* __restrict__ src, int64_t off, const Nco& nco, const XIdx& xi,
                                                 int t, int freqsync, int32_t* out)
 {
@@ -674,7 +643,7 @@ __device__ __forceinline__ void coarse_estimate(const DevTables& tb, SyncSmem& s
     if (t < TwLayout::C4) sm.o.tw[t] = tb.tw_fwd[t];
     __syncthreads();
     // the PRS useful part starts `off` samples into the window; its samples continue the NCO phase sequence
-    fft2048_from_global<EXACT, false>(src, off, v, sm.o, t, xi, tb, nco, tb.tw_fwd + TwLayout::C5);
+    fft2048_from_global(src, off, v, sm.o, t, xi, tb, nco, tb.tw_fwd + TwLayout::C5);
     if (freqsync == 1) {
         // ---- GetMiddle (:617-644), including its `sum = oldMax` assignment: moving sum of |X| over K carriers
 #pragma unroll
@@ -770,10 +739,10 @@ tii_spectra_kernel(DevTables tb, const float2* iq, int64_t stride, const int64_t
     float2 v[16];
     if (which == 0) {
         const Nco nco = make_nco(nco_frame[4 * f], nco_frame[4 * f + 1]);
-        fft2048_from_global<true, false>(iq + (int64_t)f * stride + prs_start[f], 0, v, sm, t, xi, tb, nco, tb.tw_fwd + TwLayout::C5);
+        fft2048_from_global(iq + (int64_t)f * stride + prs_start[f], 0, v, sm, t, xi, tb, nco, tb.tw_fwd + TwLayout::C5);
     } else {
         const Nco nco = make_nco(0, 0);
-        fft2048_from_global<true, false>(nulls + (int64_t)f * TNULL, TNULL - TU, v, sm, t, xi, tb, nco, tb.tw_fwd + TwLayout::C5);
+        fft2048_from_global(nulls + (int64_t)f * TNULL, TNULL - TU, v, sm, t, xi, tb, nco, tb.tw_fwd + TwLayout::C5);
     }
 #pragma unroll
     for (int c = 0; c < 16; c++) dst[t + 128 * c] = v[c];
@@ -788,10 +757,10 @@ coarse_kernel(DevTables tb, const float2* iq, int64_t stride, const int64_t* prs
     const int t = threadIdx.x, f = blockIdx.x;
     const Nco nco = make_nco(0, 0);
     const XIdx xi = make_xidx(t);
-    coarse_estimate<true>(tb, sm, iq + (int64_t)f * stride, prs_start[f], nco, xi, t, freqsync, out + f);
+    coarse_estimate(tb, sm, iq + (int64_t)f * stride, prs_start[f], nco, xi, t, freqsync, out + f);
 }
 
-template <bool EXACT, bool NCO>
+template <bool NCO>
 __global__ void __launch_bounds__(OFDM_THREADS, 5)
 find_index_kernel(DevTables tb, SyncParams p)
 {
@@ -805,7 +774,7 @@ find_index_kernel(DevTables tb, SyncParams p)
     const Nco nco = make_nco((NCO && p.nco) ? p.nco[2 * f] : 0, (NCO && p.nco) ? p.nco[2 * f + 1] : 0);
     const XIdx xi = make_xidx(t);
     float2 v[16];
-    fft2048_from_global<EXACT, false>(src, 0, v, sm.o, t, xi, tb, nco, tb.tw_fwd + TwLayout::C5);
+    fft2048_from_global(src, 0, v, sm.o, t, xi, tb, nco, tb.tw_fwd + TwLayout::C5);
     // res = X * conj(ref), written in natural order into the exchange buffer (free between the two transforms)
     float2* scratch = sm.o.xbuf;
     __syncthreads();             // pass C of the forward transform has read xbuf
@@ -814,8 +783,8 @@ find_index_kernel(DevTables tb, SyncParams p)
         const int bin = t + 128 * c;
         const float2 r = tb.prs_ref[bin];
         const float cc = r.x, d = -r.y;
-        scratch[bin] = make_float2(fsub_<EXACT>(fmul_<EXACT>(v[c].x, cc), fmul_<EXACT>(v[c].y, d)),
-                                   fadd_<EXACT>(fmul_<EXACT>(v[c].x, d), fmul_<EXACT>(v[c].y, cc)));
+        scratch[bin] = make_float2(fsub_<true>(fmul_<true>(v[c].x, cc), fmul_<true>(v[c].y, d)),
+                                   fadd_<true>(fmul_<true>(v[c].x, d), fmul_<true>(v[c].y, cc)));
     }
     __syncthreads();
     if (t < TwLayout::C4) sm.o.tw[t] = tb.tw_inv[t];
@@ -830,7 +799,7 @@ find_index_kernel(DevTables tb, SyncParams p)
 #pragma unroll
         for (int h = 0; h < 2; h++) {
             float2 y[8];
-            passA_block<EXACT, true>(x + 8 * h, y, sm.o.tw);
+            passA_block<true, true>(x + 8 * h, y, sm.o.tw);
 #pragma unroll
             for (int e = 0; e < 8; e++) sm.o.xbuf[xi.a[h] ^ e] = y[e];
         }
@@ -839,7 +808,7 @@ find_index_kernel(DevTables tb, SyncParams p)
         for (int b = 0; b < 4; b++)
 #pragma unroll
             for (int a = 0; a < 4; a++) v[a + 4 * b] = sm.o.xbuf[xi.b[a] + 32 * b];
-        passB<EXACT, true>(v, xi.kk, sm.o.tw);
+        passB<true, true>(v, xi.kk, sm.o.tw);
 #pragma unroll
         for (int b = 0; b < 4; b++)
 #pragma unroll
@@ -847,11 +816,12 @@ find_index_kernel(DevTables tb, SyncParams p)
         __syncthreads();
 #pragma unroll
         for (int c = 0; c < 16; c++) v[c] = sm.o.xbuf[(t ^ xc_of(c)) + 128 * c];
-        passC_ldg<EXACT, true>(v, t, tb.tw_inv + TwLayout::C5);
+        passC_ldg<true, true>(v, t, tb.tw_inv + TwLayout::C5);
     }
     // scale by 1/2048 (fft.cpp:146-158) and take the magnitude the way glibc's hypotf does (double sqrt, narrowed); the magnitudes go to
-    // global memory: the search over them (find_search_kernel) is a different kind of work - a 2048-step sequential sum beside a few
-    // short parallel phases - and runs as its own kernel at a much higher residency than this register-heavy transform kernel
+    // global memory: the search over them (find_search_tbp_kernel, find_search_kernel) is a different kind of work - a 2048-step
+    // sequential sum beside a few short parallel phases - and runs as its own kernel at a much higher residency than this
+    // register-heavy transform kernel
     const float factor = 1.0f / 2048.0f;
     float* cw = p.cir_work + (int64_t)f * TU;
 #pragma unroll
@@ -862,7 +832,8 @@ find_index_kernel(DevTables tb, SyncParams p)
     }
 }
 
-// findIndex, second part: the placement search over the 2048 magnitudes of one window (phasereference.cpp:93-253).  One 128-thread CTA
+// findIndex, second part: the placement search over the 2048 magnitudes of one window (phasereference.cpp:93-211) for the
+// StrongestPeak and EarliestPeakWithBinning placements (ThresholdBeforePeak, the default: find_search_tbp_kernel).  One 128-thread CTA
 // per window, 24 KB of shared memory and few registers: many windows per SM hide the sequential sum each of them carries.
 struct __align__(16) SearchSmem {
     float cir[TU];
@@ -899,55 +870,7 @@ find_search_kernel(SyncParams p)
         return acc;
     };
     int result;                 // what findIndex returns: >= 0 sample index, < 0 no synchronisation
-    if (p.placement == 0) {
-        // ---- ThresholdBeforePeak (phasereference.cpp:212-253).
-        // sliding maximum over 100 samples for i < 1948, 0 beyond (:222-238).  max() is exact, so the window maximum is
-        // built by doubling (2, 4, .. 64 samples, then max(m64[i], m64[i+36])) through the two halves of the exchange
-        // buffer instead of 100 compares per output.  The sequential sum of |.| (same order as the CPU loop, so the same
-        // float) is spread by thread 0 over the seven phases.
-        float* pk = ma;
-        float ssum = 0.f;
-        {
-            const float* srcm = sm.cir;
-            float* dstm = ma;
-#pragma unroll 1
-            for (int lvl = 0; lvl < 6; lvl++) {
-                const int sh = 1 << lvl;
-#pragma unroll
-                for (int c = 0; c < 16; c++) { const int i = t + 128 * c; dstm[i] = fmaxf(srcm[i], srcm[min(i + sh, TU - 1)]); }
-                if (t == 0) ssum = seq_sum(ssum, 74 * lvl, 74);
-                __syncthreads();
-                srcm = dstm; dstm = (dstm == ma) ? mb : ma;
-            }
-        }
-        // six levels: cir -> ma -> mb -> ma -> mb -> ma -> mb; m64 now in mb, result into ma
-        float gmax = -10000.f;
-#pragma unroll
-        for (int c = 0; c < 16; c++) {
-            const int i = t + 128 * c;
-            float m = 0.f;
-            if (i + 100 < TU) { m = fmaxf(mb[i], mb[i + 36]); gmax = fmaxf(gmax, m); }
-            pk[i] = m;
-        }
-        if (t == 0) { ssum = seq_sum(ssum, 74 * 6, TU / 4 - 74 * 6); sm.sum = ssum; }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) gmax = fmaxf(gmax, __shfl_down_sync(0xffffffffu, gmax, o));
-        if ((t & 31) == 0) sm.wmax[t >> 5] = gmax;
-        __syncthreads();
-        gmax = fmaxf(fmaxf(sm.wmax[0], sm.wmax[1]), fmaxf(sm.wmax[2], sm.wmax[3]));
-        int best = 1 << 30;
-        // `3 * sum / Tu`: float 3*sum, then / (size_t Tu converted to float)
-        if (gmax > __fdiv_rn(__fmul_rn(3.0f, sm.sum), 2048.0f)) {
-            const float thresh = gmax / 2;
-            for (int i = t; i + 100 < TU; i += OFDM_THREADS) if (pk[i + 100] > thresh) { best = min(best, i); }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_down_sync(0xffffffffu, best, o));
-        if ((t & 31) == 0) sm.wmin[t >> 5] = best;
-        __syncthreads();
-        best = min(min(sm.wmin[0], sm.wmin[1]), min(sm.wmin[2], sm.wmin[3]));
-        result = best == (1 << 30) ? -1 : best;
-    } else if (p.placement == 1) {
+    if (p.placement == 1) {
         // ---- StrongestPeak (:93-123): sequential sum, first maximum (strict >), negative score when below 3 x mean
         float mx = -10000.f; int mi = -1;
 #pragma unroll
@@ -1074,7 +997,7 @@ find_search_tbp_kernel(SyncParams p)
 
 // findIndex, third part: the coarse frequency estimate for the windows whose FIC success counter is low (ofdm-processor.cpp:397);
 // every other CTA leaves at once
-template <bool EXACT, bool NCO>
+template <bool NCO>
 __global__ void __launch_bounds__(OFDM_THREADS, 5)
 find_coarse_kernel(DevTables tb, SyncParams p)
 {
@@ -1087,7 +1010,7 @@ find_coarse_kernel(DevTables tb, SyncParams p)
     const float2* src = p.iq + (int64_t)f * p.stride + p.win_start[f];
     const Nco nco = make_nco((NCO && p.nco) ? p.nco[2 * f] : 0, (NCO && p.nco) ? p.nco[2 * f + 1] : 0);
     const XIdx xi = make_xidx(t);
-    coarse_estimate<EXACT>(tb, sm, src, result, nco, xi, t, p.freqsync, &p.coarse_out[f]);
+    coarse_estimate(tb, sm, src, result, nco, xi, t, p.freqsync, &p.coarse_out[f]);
 }
 
 } // namespace
@@ -1174,18 +1097,18 @@ void launch_coarse(const DevTables& tb, const float2* iq, int64_t stride, const 
 }
 
 // part: 0 transforms -> magnitudes, 1 placement search -> index, 2 coarse estimate where the FIC counter asks for it, -1 all three
-void launch_find_index(const DevTables& tb, const SyncParams& p, int fft_mode, cudaStream_t st, int part)
+// Time sync always uses the exact arithmetic, whatever the context's fft_mode: its integer result feeds the closed loop.
+void launch_find_index(const DevTables& tb, const SyncParams& p, cudaStream_t st, int part)
 {
     const dim3 grid(p.n), block(OFDM_THREADS);
     const bool nco = p.nco != nullptr;
-    (void)fft_mode;   // time sync always uses the exact arithmetic: its integer result feeds the closed loop
     if (part < 0 || part == 0) {
         const size_t sm = sizeof(OfdmSmem);
-        if (nco) { set_smem(find_index_kernel<true, true>, sm); find_index_kernel<true, true><<<grid, block, sm, st>>>(tb, p); }
-        else { set_smem(find_index_kernel<true, false>, sm); find_index_kernel<true, false><<<grid, block, sm, st>>>(tb, p); }
+        if (nco) { set_smem(find_index_kernel<true>, sm); find_index_kernel<true><<<grid, block, sm, st>>>(tb, p); }
+        else { set_smem(find_index_kernel<false>, sm); find_index_kernel<false><<<grid, block, sm, st>>>(tb, p); }
     }
     if (part < 0 || part == 1) {
-        if (p.placement == 0 && !p.search_generic) {
+        if (p.placement == 0) {
             cudaFuncSetAttribute(find_search_tbp_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
             find_search_tbp_kernel<<<(p.n + OFDM_THREADS / 32 - 1) / (OFDM_THREADS / 32), block, 0, st>>>(p);
         } else {
@@ -1195,8 +1118,8 @@ void launch_find_index(const DevTables& tb, const SyncParams& p, int fft_mode, c
     }
     if ((part < 0 || part == 2) && p.coarse_out) {
         const size_t sc = sizeof(SyncSmem);
-        if (nco) { set_smem(find_coarse_kernel<true, true>, sc); find_coarse_kernel<true, true><<<grid, block, sc, st>>>(tb, p); }
-        else { set_smem(find_coarse_kernel<true, false>, sc); find_coarse_kernel<true, false><<<grid, block, sc, st>>>(tb, p); }
+        if (nco) { set_smem(find_coarse_kernel<true>, sc); find_coarse_kernel<true><<<grid, block, sc, st>>>(tb, p); }
+        else { set_smem(find_coarse_kernel<false>, sc); find_coarse_kernel<false><<<grid, block, sc, st>>>(tb, p); }
     }
 }
 

@@ -14,7 +14,7 @@
 
 namespace dabb {
 
-constexpr int VIT_GROUP_CW = 128;        // codewords per CTA of the decoder kernel (viterbi.cu VIT_THREADS)
+constexpr int VIT_GROUP_CW = 128;        // codewords per CTA of the decoder kernel (viterbi.cu defines VIT_THREADS as this)
 
 // one CTA of a grouped launch
 struct VitGroup {

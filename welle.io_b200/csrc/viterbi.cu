@@ -120,10 +120,7 @@ __global__ void clamp_copy_kernel(const int8_t* src, int8_t* dst, int64_t n)
 }
 
 // ------------------------------------------------------------------------------------------------ the decoder
-#ifndef VIT_THREADS_N
-#define VIT_THREADS_N 128
-#endif
-constexpr int VIT_THREADS = VIT_THREADS_N;     // codewords per CTA
+constexpr int VIT_THREADS = VIT_GROUP_CW;     // codewords per CTA (vit_groups.cuh: the grouped schedule's descriptors hold as many)
 constexpr int VIT_MIN_CTAS = 512 / VIT_THREADS;   // 512 threads of 128 registers per SM
 constexpr int VIT_ROW_PITCH = 144;      // 128 B of softbits + 16 B pad (rows stay 16-byte aligned for the bulk copies)
 constexpr int VIT_STAGE_BYTES = VIT_THREADS * VIT_ROW_PITCH;
@@ -277,7 +274,7 @@ __device__ __forceinline__ void viterbi_cta(const ViterbiParams& p, const int bl
             for (int k = 0; k < 6; k++) w[k] = wn[k];
             if (gq < 3 && g + 1 < groups) expand(gq + 1, wn);
             uint32_t d[12];
-            vit_six_steps(Q, w, d, p.one);
+            vit_six_steps(Q, w, d);
             if (have) {
 #pragma unroll
                 for (int k = 0; k < 6; k++) dec[(int64_t)(6 * g + k) * VIT_THREADS] = make_uint2(d[2 * k], d[2 * k + 1]);
@@ -362,9 +359,8 @@ template <bool GROUPED> void launch_viterbi_t(const ViterbiParams& p, const int 
     viterbi_kernel<GROUPED><<<blocks, VIT_THREADS, sizeof(VitSmem), st>>>(p);
 }
 
-void launch_viterbi(const ViterbiParams& p_in, cudaStream_t st)
+void launch_viterbi(const ViterbiParams& p, cudaStream_t st)
 {
-    ViterbiParams p = p_in; p.one = 1u;
     if (p.groups) launch_viterbi_t<true>(p, p.n_groups, st);
     else launch_viterbi_t<false>(p, (p.n_cw + VIT_THREADS - 1) / VIT_THREADS, st);
 }

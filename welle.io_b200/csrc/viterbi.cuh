@@ -54,7 +54,6 @@ struct ViterbiParams {
     const uint32_t* prbs_words;       // energy-dispersal sequence packed like the output (or nullptr)
     const int32_t* valid;             // optional per-codeword flag
     TraceBuf trace; uint32_t trace_kind;    // optional CTA timeline (common.cuh)
-    uint32_t one;                     // = 1 (set by the launcher; keeps a multiply-add opaque to the assembler, see viterbi_core.cuh)
 };
 
 

@@ -71,10 +71,6 @@ VIT_HD uint32_t vminu16x2(uint32_t a, uint32_t b)
 #endif
 }
 
-#if defined(__CUDA_ARCH__)
-// a * b + c as one IMAD whatever the compiler thinks of the operands (b is passed through a register the assembler cannot see through)
-__device__ __forceinline__ uint32_t vit_mad(uint32_t a, uint32_t b, uint32_t c) { uint32_t r; asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c)); return r; }
-#endif
 // per-half signed 16-bit minimum (SASS: VIMNMX.S16x2)
 VIT_HD uint32_t vmin16(uint32_t a, uint32_t b)
 {
@@ -143,9 +139,8 @@ template <int DELTA> VIT_HD void vit_mc(uint32_t w, uint32_t (&MC)[8])
 
 // One ACS step from layout L_B to L_{(B+1)%6}.  Q: 32 packed metric registers; dlo/dhi: decision bits of new states
 // 0..31 / 32..63.
-template <int B> VIT_HD void vit_acs(uint32_t (&Q)[32], const uint32_t w, uint32_t& dlo, uint32_t& dhi, const uint32_t one)
+template <int B> VIT_HD void vit_acs(uint32_t (&Q)[32], const uint32_t w, uint32_t& dlo, uint32_t& dhi)
 {
-    const uint32_t vit_minus_one = 0u - one; (void)vit_minus_one;
     uint32_t N[32];
     // Decisions without predicates.  For a packed pair (a, b) of candidate metrics (every half in [0, 0x7FFF]) t = a + 0x7FFF7FFF - b has
     // bit 15 / 31 set exactly where b wins strictly ((a - b) > 0: ties keep the a = old[i] branch, viterbi.cpp:263-275) and no carry
@@ -156,13 +151,7 @@ template <int B> VIT_HD void vit_acs(uint32_t (&Q)[32], const uint32_t w, uint32
     // Decision layout of a step: group g (0..15) = the two packed minima that share their input registers, byte lane l (0..3) as listed
     // below; decision bit at word g >> 3, bit 8 l + (g & 7) (vit_dec_pos<B> is the inverse map for the traceback).
     uint32_t W[2] = {0u, 0u};
-#if defined(VIT_T_FMA) && defined(__CUDA_ARCH__)
-    // the same word on the multiply-add pipe: (a + C) is one more two-input add (IMAD.IADD) and t = b * (-1) + (a + C) an IMAD, instead of
-    // one three-input IADD3 on the ALU pipe, which already carries the packed minima, the PRMTs and the LOP3s at half rate
-#define VIT_T(a, b) vit_mad((b), vit_minus_one, vit_mad((a), one, 0x7FFF7FFFu))
-#else
 #define VIT_T(a, b) ((a) + 0x7FFF7FFFu - (b))
-#endif
 #define VIT_PUT(g, t1, t2) do { W[(g) >> 3] |= vit_signbytes(t1, t2) & (0x01010101u << ((g) & 7)); } while (0)
     if constexpr (B < 5) {
         constexpr int delta = vit_pat(1 << B);   // pattern change when butterfly bit B flips
@@ -226,14 +215,14 @@ VIT_HD void vit_normalize(uint32_t (&Q)[32])
 }
 
 // six steps: words w[0..5] hold the symbols, dec[2*s], dec[2*s+1] receive the decision words
-VIT_HD void vit_six_steps(uint32_t (&Q)[32], const uint32_t w[6], uint32_t dec[12], const uint32_t one = 1u)
+VIT_HD void vit_six_steps(uint32_t (&Q)[32], const uint32_t w[6], uint32_t dec[12])
 {
-    vit_acs<0>(Q, w[0], dec[0], dec[1], one);
-    vit_acs<1>(Q, w[1], dec[2], dec[3], one);
-    vit_acs<2>(Q, w[2], dec[4], dec[5], one);
-    vit_acs<3>(Q, w[3], dec[6], dec[7], one);
-    vit_acs<4>(Q, w[4], dec[8], dec[9], one);
-    vit_acs<5>(Q, w[5], dec[10], dec[11], one);
+    vit_acs<0>(Q, w[0], dec[0], dec[1]);
+    vit_acs<1>(Q, w[1], dec[2], dec[3]);
+    vit_acs<2>(Q, w[2], dec[4], dec[5]);
+    vit_acs<3>(Q, w[3], dec[6], dec[7]);
+    vit_acs<4>(Q, w[4], dec[8], dec[9]);
+    vit_acs<5>(Q, w[5], dec[10], dec[11]);
 }
 
 // ---- de-puncturing inside the decoder kernel -------------------------------------------------------------------------------

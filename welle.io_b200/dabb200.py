@@ -11,7 +11,7 @@ import weakref
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("DABB_LIB") or os.path.join(HERE, "libdab_b200.so")   # DABB_LIB: build-variant experiments only
+LIB_PATH = os.environ.get("DABB_LIB") or os.path.join(HERE, "libdab_b200.so")   # DABB_LIB: another build of the library, e.g. the parent's for scripts/gpu_ab.sh
 
 L, K, TU, TS, TG, TNULL, TF = 76, 1536, 2048, 2552, 504, 2656, 196608
 SOFT_PER_FRAME = 75 * 3072
