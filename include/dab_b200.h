@@ -137,6 +137,39 @@ typedef struct {
     int32_t reserved;
 } dabb_clock_result;
 
+/* Diversity reception (replaces: none; the reference is one receiver with one input).  Coherent multi-channel receivers record one file
+ * per antenna on a shared sample clock; decoded as neighbouring streams of one context, the antennas of one capture can be combined.
+ * dabb_set_combining groups streams: leader is a HOST array of n == n_streams entries; leader[s] == s means stream s is alone or leads a
+ * group, any other value is the stream whose group s joins.  Every entry must satisfy leader[leader[s]] == leader[s], and a group has at
+ * most DABB_MAX_BRANCHES members, its leader included; NULL dissolves every group.  A malformed table (an index out of range, a chain, an
+ * oversized group, a wrong n) returns DABB_E_ARG and changes nothing.  Like a select call, the function waits for outstanding work and
+ * takes effect from the next step; dabb_stream_reset does not change the grouping.  The members of a group must share one logical sample
+ * axis (buf_start), as the files of one coherent capture do.
+ * In a step where leader L decodes a frame (DABB_FRAME_DECODED):
+ *   A_x = buf_start[x] + the start of x's phase reference symbol in its buffer, the symbol's absolute position;
+ *   N_x = the mean of |y|^2 over the 2656 samples of the null symbol that ends x's frame window, NCO applied (tap 3's samples): for i in
+ *         ascending order the partial sums t = i mod 256 of Re^2 + Im^2, then the 256 partial sums in order, divided by 2656 (fp32);
+ *   member b contributes when it also decoded a frame in this step, |A_b - A_L| <= 504 and N_b is finite and > 0; L always contributes
+ *   (alone, when N_L itself is 0 or not finite);
+ *   for every data symbol l the leader's decoders read and every carrier k, R = sum over the contributors in ascending stream index of
+ *   r1_b[l][k] / N_b in fp32 (each division and addition rounded), r1_b the product b's own demap reads (derotated under
+ *   DABB_CLOCK_TRACK); the leader's softbits are the context's demap of R: DABB_DEMAP_REFERENCE trunc(-Re/Im(R) 127 / l1(R)),
+ *   DABB_DEMAP_WEIGHTED with G taken over the combined levels (per thread of 128 in ascending carrier order, the 128 sums in order).
+ * The result depends neither on the batch size, ofdm_groups nor the tail split.  When no other member contributes the leader's softbits
+ * are its own, bit for bit.  Every member other than the leader decodes exactly as it would ungrouped (its FIBs, logical frames, BER,
+ * TII and clock outputs are unchanged), so each antenna's own result stays available.  The leader's FIC, sub-channels and tap 10 read the
+ * combined softbits, and so does tap 0 of a leader (for every symbol); taps 2 and 3 keep every stream's own values.  A context that never
+ * forms a group of two or more allocates nothing for it and runs exactly what it runs without this call. */
+enum { DABB_MAX_BRANCHES = 8 };
+int dabb_set_combining(dabb_ctx* ctx, const int32_t* leader, int32_t n);
+/* one stream in one step: tap 12 */
+typedef struct {
+    int32_t members;            /* contributors of this step (the leader included); 0 for a non-leader or a step without a frame */
+    uint32_t mask;              /* bit i: the i-th member of the group in ascending stream order contributed */
+    float noise;                /* this stream's N, or 0 when it was not computed (not grouped, or no frame) */
+    int32_t reserved;
+} dabb_combine_result;
+
 /* Channel bit errors of one stream in one step: tap 10, while dabb_options.count_bit_errors is set.  Per codeword (a FIC block of 768
  * bits, or a logical frame of 24 * bitrate bits) the decoded bits before energy dispersal (the output bytes MSB first, XOR the PRBS; 6
  * zero tail bits) are re-encoded with the K=7 rate-1/4 mother code and punctured like the codeword's protection (FIC: 21 x PI_16,
@@ -311,7 +344,9 @@ int dabb_profile_read(dabb_ctx* ctx, char* json_out, size_t cap);
  *  10 = dabb_ber_result [n_streams] of the last step (all zero when that step ran with count_bit_errors off); DABB_E_STATE until
  *       dabb_options.count_bit_errors has been set once
  *  11 = dabb_clock_result [n_streams] of the last step (all zero when that step ran with sample_clock OFF); DABB_E_STATE until
- *       dabb_options.sample_clock has been set to DABB_CLOCK_TRACK once */
+ *       dabb_options.sample_clock has been set to DABB_CLOCK_TRACK once
+ *  12 = dabb_combine_result [n_streams] of the last step (all zero when that step ran without a group); DABB_E_STATE until
+ *       dabb_set_combining has formed a group of two or more streams once */
 int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes);
 
 /* ---------------------------------------------------------------------------------------------------------

@@ -157,6 +157,15 @@ struct dabb_ctx {
     // without keep_taps: [S][OFDM_MASK_WORDS] the OFDM symbols each stream's decoders read (ofdm_mask.cuh), rebuilt by every select and
     // remove call; the OFDM launch of the last step, which tap 0 repeats over every symbol when soft_partial says it skipped some
     DevBuf<uint32_t> d_symmask; OfdmParams soft_op{}; bool soft_partial = false;
+    // diversity combining (dabb_set_combining, combine.cu), all empty until a group of two or more forms (comb_on): the leader table; per
+    // group its members and their r1 rows (d_comb_groups) and the (group, symbol) items of combine_kernel (d_comb_items); per stream its
+    // group or -1 (d_comb_gid).  Without keep_taps the OFDM kernel stores the grouped streams' r1 of their leader's symbols in d_comb_r1
+    // (row d_comb_row[s], the symbols d_comb_lmask[s] marks); with it combine_kernel reads tap 2's d_r1.  d_comb_groups_full /
+    // d_comb_row_full: the rows of every symbol, for the tap-0 repeat.  d_comb_res: tap 12, kept once allocated; comb_op: the last
+    // step's combine launch
+    std::vector<int32_t> h_leader; bool comb_on = false; int comb_n_groups = 0, comb_n_items = 0, comb_n_grouped = 0;
+    DevBuf<CombGroup> d_comb_groups, d_comb_groups_full; DevBuf<CombItem> d_comb_items; DevBuf<int32_t> d_comb_gid, d_comb_row, d_comb_row_full;
+    DevBuf<uint32_t> d_comb_lmask; DevBuf<float2> d_comb_r1; DevBuf<dabb_combine_result> d_comb_res; CombParams comb_op{};
 };
 
 namespace {
@@ -399,6 +408,21 @@ __global__ void advance_kernel(StreamState* st, StepScratch* scr, int S, int gro
     scr[s] = c;
 }
 
+// sample i of the null symbol that follows stream s's frame, read with the NCO at coarse + fine (after this frame's fine update); 0 when
+// the stream decoded no frame or the sample is outside its buffer (p0: the null symbol's first sample relative to the buffer)
+__device__ __forceinline__ float2 null_sample(const StepScratch& c, const float2* iq, int64_t stride, int s, int64_t p0, int64_t buf_len, const float2* osc, bool mix, int i)
+{
+    float2 v = make_float2(0.f, 0.f);
+    if (c.active && p0 >= 0 && p0 + i < buf_len) {
+        v = iq[(int64_t)s * stride + p0 + i];
+        if (mix) {
+            const float2 o = osc[mod_rate((int64_t)c.null_lp - (int64_t)(i + 1) * c.null_ph)];
+            v = make_float2(__fsub_rn(__fmul_rn(v.x, o.x), __fmul_rn(v.y, o.y)), __fadd_rn(__fmul_rn(v.x, o.y), __fmul_rn(v.y, o.x)));
+        }
+    }
+    return v;
+}
+
 // diagnostics tap: the null symbol as OFDMProcessor::run hands it to onNewNullSymbol (ofdm-processor.cpp:462-469): T_null
 // samples read with the NCO at coarse + fine (after this frame's fine update)
 __global__ void null_tap_kernel(const StepScratch* scr, const float2* iq, int64_t stride, const int64_t* buf_start, int64_t buf_len, const float2* osc, float2* out)
@@ -408,17 +432,29 @@ __global__ void null_tap_kernel(const StepScratch* scr, const float2* iq, int64_
     float2* dst = out + (int64_t)s * TNULL;
     const int64_t p0 = c.null_pos - buf_start[s];
     const bool mix = c.null_lp != 0 || c.null_ph != 0;
-    for (int i = threadIdx.x; i < TNULL; i += blockDim.x) {
-        float2 v = make_float2(0.f, 0.f);
-        if (c.active && p0 >= 0 && p0 + i < buf_len) {
-            v = iq[(int64_t)s * stride + p0 + i];
-            if (mix) {
-                const float2 o = osc[mod_rate((int64_t)c.null_lp - (int64_t)(i + 1) * c.null_ph)];
-                v = make_float2(__fsub_rn(__fmul_rn(v.x, o.x), __fmul_rn(v.y, o.y)), __fadd_rn(__fmul_rn(v.x, o.y), __fmul_rn(v.y, o.x)));
-            }
-        }
-        dst[i] = v;
+    for (int i = threadIdx.x; i < TNULL; i += blockDim.x) dst[i] = null_sample(c, iq, stride, s, p0, buf_len, osc, mix, i);
+}
+
+// diversity combining, lane A after advance_kernel: the noise power N (combine_core.cuh) of every grouped stream that decoded a frame,
+// from the same null-symbol samples as tap 3; every stream's tap-12 record of the step starts as {0, 0, N or 0}
+__global__ void __launch_bounds__(dabb_comb::NULL_THREADS)
+null_power_kernel(const StepScratch* scr, const int32_t* gid, const float2* iq, int64_t stride, const int64_t* buf_start, int64_t buf_len, const float2* osc,
+                  dabb_combine_result* res)
+{
+    __shared__ float part[dabb_comb::NULL_THREADS];
+    const int s = blockIdx.x, t = threadIdx.x;
+    const StepScratch c = scr[s];
+    if (gid[s] < 0 || !c.active) { if (t == 0) res[s] = dabb_combine_result{0, 0u, 0.f, 0}; return; }
+    const int64_t p0 = c.null_pos - buf_start[s];
+    const bool mix = c.null_lp != 0 || c.null_ph != 0;
+    float a = 0.f;
+    for (int i = t; i < TNULL; i += dabb_comb::NULL_THREADS) {
+        const float2 v = null_sample(c, iq, stride, s, p0, buf_len, osc, mix, i);
+        a = __fadd_rn(a, __fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y)));       // dabb_comb::null_partial
     }
+    part[t] = a;
+    __syncthreads();
+    if (t == 0) res[s] = dabb_combine_result{0, 0u, dabb_comb::null_noise(part), 0};
 }
 
 // lane B, after FIC / MSC / RS of the frame: decoder-side state and the result record
@@ -619,22 +655,102 @@ int repitch(dabb_ctx* ctx, DevBuf<uint8_t>& b, size_t rows, size_t old_pitch, si
     return DABB_OK;
 }
 
-// the symbol masks of streams [first, first + count) from their slots (h_slots), uploaded on the context's stream; the caller synchronises
-// it before the host vector is gone (the copy is from pageable memory, so it is staged before cudaMemcpyAsync returns anyway)
+// the symbols stream s's own decoders read (ofdm_mask.cuh), from its slots (h_slots)
+void own_symmask(dabb_ctx* ctx, int s, uint32_t* m)
+{
+    const int ns = ctx->n_slots;
+    OfdmMaskSlot sl[DABB_MAX_SUBCH];
+    for (int k = 0; k < ns; k++) {
+        const MscSlotState& st = ctx->h_slots[(size_t)s * ns + k];
+        sl[k] = OfdmMaskSlot{st.enabled, st.start_cu, st.frag / 64};
+    }
+    build_ofdm_mask(sl, ns, m);
+}
+
+// the symbol masks of streams [first, first + count), uploaded on the context's stream; the caller synchronises it before the host vector
+// is gone (the copy is from pageable memory, so it is staged before cudaMemcpyAsync returns anyway).  While streams are grouped every
+// stream's mask is rebuilt: a member also transforms the symbols its leader reads, so that combine_kernel has their products.
 int upload_symmask(dabb_ctx* ctx, int first, int count)
 {
     if (!ctx->d_symmask) return DABB_OK;
-    const int ns = ctx->n_slots;
+    if (ctx->comb_on) { first = 0; count = ctx->S; }
     std::vector<uint32_t> m((size_t)count * OFDM_MASK_WORDS);
-    for (int i = 0; i < count; i++) {
-        OfdmMaskSlot sl[DABB_MAX_SUBCH];
-        for (int k = 0; k < ns; k++) {
-            const MscSlotState& st = ctx->h_slots[(size_t)(first + i) * ns + k];
-            sl[k] = OfdmMaskSlot{st.enabled, st.start_cu, st.frag / 64};
+    for (int i = 0; i < count; i++) own_symmask(ctx, first + i, m.data() + (size_t)i * OFDM_MASK_WORDS);
+    if (ctx->comb_on) {
+        std::vector<uint32_t> own(m);
+        for (int s = 0; s < ctx->S; s++) {
+            const int L = ctx->h_leader[(size_t)s];
+            for (int w = 0; w < OFDM_MASK_WORDS; w++) m[(size_t)s * OFDM_MASK_WORDS + w] |= own[(size_t)L * OFDM_MASK_WORDS + w];
         }
-        build_ofdm_mask(sl, ns, m.data() + (size_t)i * OFDM_MASK_WORDS);
     }
     CK(cudaMemcpyAsync(ctx->d_symmask + (size_t)first * OFDM_MASK_WORDS, m.data(), m.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+    return DABB_OK;
+}
+
+template <typename T> int upload(dabb_ctx* ctx, DevBuf<T>& b, const std::vector<T>& h)
+{
+    int rc;
+    if ((rc = alloc(ctx, b, h.size()))) return rc;
+    if (!h.empty()) CK(cudaMemcpyAsync(b, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+    return DABB_OK;
+}
+
+// the tables of diversity combining from h_leader and the leaders' symbol masks (the caller has run sync_all).  Each group of two or more
+// streams combines the data symbols its leader's decoders read (every symbol with keep_taps); without keep_taps its members' r1 rows of
+// those symbols lie one after the other in d_comb_r1.  `regroup`: the grouping itself changed, so the tap-0 repeat's rows are rebuilt too
+// and the last step's combination is not repeated.  No group: every table is freed (tap 12's records stay).
+int rebuild_comb(dabb_ctx* ctx, bool regroup)
+{
+    const int S = ctx->S, W = OFDM_MASK_WORDS;
+    const bool taps = !ctx->d_symmask;
+    std::vector<std::vector<int32_t>> members(ctx->h_leader.empty() ? 0 : (size_t)S);
+    for (int s = 0; s < (int)members.size(); s++) members[(size_t)ctx->h_leader[(size_t)s]].push_back(s);
+    std::vector<CombGroup> groups, full; std::vector<CombItem> items;
+    std::vector<int32_t> gid((size_t)S, -1), row((size_t)S, -1), row_full((size_t)S, -1); std::vector<uint32_t> lmask((size_t)S * W, 0u);
+    int64_t rows = 0; int rank = 0;
+    for (int L = 0; L < (int)members.size(); L++) {
+        const auto& mb = members[(size_t)L];
+        if (mb.size() < 2) continue;
+        uint32_t m[OFDM_MASK_WORDS] = {0u, 0u, 0u, 0u};
+        if (taps) for (int l = 1; l <= 75; l++) m[l >> 5] |= 1u << (l & 31);
+        else own_symmask(ctx, L, m);
+        int nsym = 0;
+        for (int w = 0; w < W; w++) for (uint32_t x = m[w]; x; x &= x - 1) nsym++;
+        CombGroup g{}, gf{};
+        g.n = gf.n = (int32_t)mb.size();
+        const int gi = (int)groups.size();
+        for (int i = 0; i < g.n; i++) {
+            const int s = mb[(size_t)i];
+            if (s == L) g.lpos = gf.lpos = i;
+            g.stream[i] = gf.stream[i] = s;
+            g.row[i] = taps ? 75 * s : (int32_t)(rows + (int64_t)i * nsym);
+            gf.row[i] = 75 * (rank + i);
+            gid[(size_t)s] = gi; row[(size_t)s] = g.row[i]; row_full[(size_t)s] = gf.row[i];
+            for (int w = 0; w < W; w++) lmask[(size_t)s * W + w] = m[w];
+        }
+        int col = 0;
+        for (int l = 1; l <= 75; l++)
+            if ((m[l >> 5] >> (l & 31)) & 1u) { items.push_back(CombItem{gi, l, taps ? l - 1 : col, col == 0}); col++; }
+        rows += (int64_t)g.n * nsym; rank += g.n;
+        groups.push_back(g); full.push_back(gf);
+    }
+    ctx->comb_on = !groups.empty();
+    if (regroup) ctx->comb_op = CombParams{};
+    if (!ctx->comb_on) {
+        ctx->d_comb_groups.reset(); ctx->d_comb_groups_full.reset(); ctx->d_comb_items.reset(); ctx->d_comb_gid.reset(); ctx->d_comb_row.reset();
+        ctx->d_comb_row_full.reset(); ctx->d_comb_lmask.reset(); ctx->d_comb_r1.reset();
+        ctx->comb_n_groups = ctx->comb_n_items = ctx->comb_n_grouped = 0;
+        return DABB_OK;
+    }
+    int rc;
+    if ((rc = upload(ctx, ctx->d_comb_groups, groups)) || (rc = upload(ctx, ctx->d_comb_items, items)) || (rc = upload(ctx, ctx->d_comb_gid, gid))) return rc;
+    if (!taps) {
+        if ((rc = upload(ctx, ctx->d_comb_row, row)) || (rc = upload(ctx, ctx->d_comb_lmask, lmask))) return rc;
+        if ((size_t)rows * KC > ctx->d_comb_r1.size() || (size_t)rows * KC * 2 < ctx->d_comb_r1.size()) { ctx->d_comb_r1.reset(); if ((rc = alloc(ctx, ctx->d_comb_r1, (size_t)rows * KC))) return rc; }
+        if (regroup && ((rc = upload(ctx, ctx->d_comb_groups_full, full)) || (rc = upload(ctx, ctx->d_comb_row_full, row_full)))) return rc;
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->comb_n_groups = (int)groups.size(); ctx->comb_n_items = (int)items.size(); ctx->comb_n_grouped = rank;
     return DABB_OK;
 }
 
@@ -670,7 +786,7 @@ int set_slot_streams(dabb_ctx* ctx, int slot, int first, int count, const MscSlo
     }
     set_slot_kernel<<<(count + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_slots, ns, slot, first, count, v);
     for (int i = first; i < first + count; i++) ctx->h_slots[(size_t)i * ns + slot] = v;
-    if ((rc = upload_symmask(ctx, first, count))) return rc;
+    if ((rc = upload_symmask(ctx, first, count)) || (ctx->comb_on && (rc = rebuild_comb(ctx, false)))) return rc;
     { int rc_ = check_launch(ctx, "set_slot_kernel"); cudaStreamSynchronize(ctx->stream); return rc_; }
 }
 
@@ -903,6 +1019,35 @@ int dabb_remove_subchannel(dabb_ctx* ctx, int32_t first, int32_t count, int32_t 
     return set_slot_streams(ctx, slot, first, count, MscSlotState{});
 }
 
+int dabb_set_combining(dabb_ctx* ctx, const int32_t* leader, int32_t n)
+{
+    if (!ctx) return DABB_E_ARG;
+    const int S = ctx->S;
+    std::vector<int32_t> L((size_t)S);
+    if (leader) {
+        if (n != S) { ctx->err = "dabb_set_combining: the table needs n_streams entries"; return DABB_E_ARG; }
+        std::vector<int> size((size_t)S, 0);
+        for (int s = 0; s < S; s++) {
+            const int32_t v = leader[s];
+            if (v < 0 || v >= S) { ctx->err = "dabb_set_combining: leader[" + std::to_string(s) + "] is not a stream"; return DABB_E_ARG; }
+            if (leader[v] != v) { ctx->err = "dabb_set_combining: leader[" + std::to_string(s) + "] is not a leader (leader[leader[s]] != leader[s])"; return DABB_E_ARG; }
+            if (++size[(size_t)v] > DABB_MAX_BRANCHES) { ctx->err = "dabb_set_combining: a group has more than DABB_MAX_BRANCHES members"; return DABB_E_ARG; }
+            L[(size_t)s] = v;
+        }
+    } else
+        for (int s = 0; s < S; s++) L[(size_t)s] = s;
+    cudaSetDevice(ctx->device);
+    sync_all(ctx);
+    const bool was = ctx->comb_on;
+    ctx->h_leader = L;
+    int rc;
+    if ((rc = rebuild_comb(ctx, true))) return rc;
+    if (ctx->comb_on && !ctx->d_comb_res && (rc = dalloc(ctx, ctx->d_comb_res, (size_t)S))) return rc;
+    if ((was || ctx->comb_on) && (rc = upload_symmask(ctx, 0, S))) return rc;
+    CK(cudaStreamSynchronize(ctx->stream));
+    return DABB_OK;
+}
+
 
 static int run_fic(dabb_ctx* ctx, const int8_t* soft, int64_t soft_stride, const int32_t* active, int n_frames, uint8_t* fibs, int32_t* crc, cudaStream_t st, uint2* dec)
 {
@@ -1013,6 +1158,7 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     op.trace = ctx->trace;
     op.n_full = S - ctx->tail_frames; op.tail_groups = ctx->tail_frames ? OFDM_TAIL_GROUPS : 1; op.fc_pitch = ctx->fc_pitch; op.nco_fast = ctx->nco_fast; op.weighted = ctx->soft_demap == DABB_DEMAP_WEIGHTED;
     op.symmask = ctx->d_symmask; op.clock = d_clock_frame;
+    if (ctx->comb_on && !ctx->keep_taps) { op.r1 = ctx->d_comb_r1; op.r1_row = ctx->d_comb_row; op.r1_lmask = ctx->d_comb_lmask; }     // the grouped streams' r1 of their leader's symbols
     launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, A);
     ctx->soft_op = op; ctx->soft_partial = op.symmask != nullptr;
     if ((rc = check_launch(ctx, "ofdm_demod_kernel"))) return rc;
@@ -1036,6 +1182,17 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         }
     }
     if (!ctx->decode_tii && ctx->d_tii_res) CK(cudaMemsetAsync(ctx->d_tii_res, 0, sizeof(dabb_tii_result) * S, A));     // tap 9: nothing analysed in this step
+    // diversity combining: the members' noise powers, then the leaders' softbits from their groups' products
+    if (ctx->comb_on) {
+        null_power_kernel<<<S, dabb_comb::NULL_THREADS, 0, A>>>(scr, ctx->d_comb_gid, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, ctx->d_comb_res);
+        if ((rc = check_launch(ctx, "null_power_kernel"))) return rc;
+        CombParams cp{}; cp.groups = ctx->d_comb_groups; cp.items = ctx->d_comb_items; cp.n_items = ctx->comb_n_items; cp.r1 = ctx->keep_taps ? ctx->d_r1.get() : ctx->d_comb_r1.get();
+        cp.active = d_active; cp.prs = d_prs; cp.buf_start = ctx->d_buf_start; cp.res = ctx->d_comb_res.get(); cp.soft = d_soft; cp.soft_stride = DABB_SOFT_PER_FRAME;
+        cp.weighted = ctx->soft_demap == DABB_DEMAP_WEIGHTED;
+        launch_combine(cp, A);
+        if ((rc = check_launch(ctx, "combine_kernel"))) return rc;
+        ctx->comb_op = cp;
+    } else if (ctx->d_comb_res) CK(cudaMemsetAsync(ctx->d_comb_res, 0, sizeof(dabb_combine_result) * S, A));     // tap 12: no group in this step
     if (!serial) { CK(cudaEventRecord(ctx->evA[par], A)); CK(cudaStreamWaitEvent(B, ctx->evA[par], 0)); }
     // ---------------- lane B: FIC chain forked onto its own stream, MSC chain per slot (longest first), then the result record.
     // (One fused Viterbi launch over FIC + MSC codewords was measured slower: 1.44 ms vs 0.34 + 1.02 ms.)
@@ -1209,9 +1366,22 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
         // the last step demapped only the symbols its decoders read: repeat its OFDM launch over every symbol, from the same input and
         // per-frame parameters, writing nothing but the softbits (the symbols it did demap get the same bytes again)
         OfdmParams op = ctx->soft_op;
-        op.symmask = nullptr; op.r1 = nullptr; op.freqcorr = nullptr; op.level = nullptr; op.snr = nullptr; op.trace = TraceBuf{nullptr, nullptr, 0};
+        op.symmask = nullptr; op.r1 = nullptr; op.r1_row = nullptr; op.r1_lmask = nullptr; op.freqcorr = nullptr; op.level = nullptr; op.snr = nullptr; op.trace = TraceBuf{nullptr, nullptr, 0};
+        // a step that combined: the grouped streams' r1 of every symbol into a temporary, then the combination over every symbol
+        DevBuf<float2> full;
+        const bool comb = ctx->comb_op.n_items > 0 && ctx->d_comb_groups_full;
+        if (comb) {
+            int rc;
+            if ((rc = alloc(ctx, full, (size_t)ctx->comb_n_grouped * 75 * KC))) return rc;
+            op.r1 = full; op.r1_row = ctx->d_comb_row_full;
+        }
         launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, ctx->stream);
         CK(cudaGetLastError());
+        if (comb) {
+            CombParams cp = ctx->comb_op; cp.groups = ctx->d_comb_groups_full; cp.items = nullptr; cp.n_items = ctx->comb_n_groups * 75; cp.r1 = full;
+            launch_combine(cp, ctx->stream);
+            CK(cudaGetLastError());
+        }
         CK(cudaStreamSynchronize(ctx->stream));
         ctx->soft_partial = false;
     }
@@ -1234,6 +1404,10 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
     if (what == 11) {
         if (!ctx->d_clock_res) { ctx->err = "tap 11 needs dabb_options.sample_clock to have been set"; return DABB_E_STATE; }
         const size_t n = sizeof(dabb_clock_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_clock_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
+    }
+    if (what == 12) {
+        if (!ctx->d_comb_res) { ctx->err = "tap 12 needs dabb_set_combining to have formed a group"; return DABB_E_STATE; }
+        const size_t n = sizeof(dabb_combine_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_comb_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
     }
     if (what == 4 && ctx->d_tii && ctx->d_null && ctx->decode_tii) { const size_t n = (size_t)ctx->S * 2 * TU * 8; CK(cudaMemcpy(host_out, ctx->d_tii, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 3 && ctx->d_null) { const size_t n = (size_t)ctx->S * TNULL * 8; CK(cudaMemcpy(host_out, ctx->d_null, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }

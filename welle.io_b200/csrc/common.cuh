@@ -9,6 +9,7 @@
 #include "chan_core.cuh"
 #include "ofdm_mask.cuh"
 #include "clock_core.cuh"
+#include "combine_core.cuh"
 
 namespace dabb {
 
@@ -63,6 +64,10 @@ struct OfdmParams {
     const uint32_t* symmask;                     // [n][OFDM_MASK_WORDS] the symbols each frame demaps (ofdm_mask.cuh), or nullptr: all of them
     TraceBuf trace;                              // rec == nullptr: off
     const float* clock;                          // [n] sample-clock ppm whose phase ramp the demap removes (clock_core.cuh), or nullptr: none
+    // where the TAP instances store r1 (see r1_dst in ofdm.cu): nullptr = the constellation tap's layout [n][75][1536]; else a row index per
+    // frame (< 0: none) and optionally [n][OFDM_MASK_WORDS] the symbols that get a row (diversity combining, combine.cu)
+    const int32_t* r1_row;
+    const uint32_t* r1_lmask;
 };
 
 struct SyncParams {
@@ -86,6 +91,29 @@ void launch_find_index(const DevTables& tb, const SyncParams& p, cudaStream_t st
 void launch_tii_spectra(const DevTables& tb, const float2* iq, int64_t stride, const int64_t* prs_start, const int32_t* nco_frame, const int32_t* active,
                         const float2* nulls, float2* out, int n, cudaStream_t st);
 void launch_coarse(const DevTables& tb, const float2* iq, int64_t stride, const int64_t* prs_start, int n, int freqsync, int32_t* out, cudaStream_t st);
+
+// ---- diversity combining (combine.cu, combine_core.cuh) ----
+// one group of streams of a context (dabb_set_combining): members in ascending stream order, the leader at lpos; member i's r1 of the
+// leader's j-th combined symbol is row row[i] + j of CombParams::r1
+struct CombGroup {
+    int32_t n, lpos;
+    int32_t stream[dabb_comb::MAX_BRANCHES];
+    int32_t row[dabb_comb::MAX_BRANCHES];
+};
+// one CTA of combine_kernel: data symbol sym (1..75) of a group, in column col of the members' rows; `first`: the group's first item,
+// which writes the leader's tap-12 record
+struct CombItem { int32_t group, sym, col, first; };
+struct CombParams {
+    const CombGroup* groups;
+    const CombItem* items; int n_items;          // items == nullptr: every symbol of every group, item i = (i / 75, i % 75 + 1, i % 75)
+    const float2* r1;                            // rows of KC products (logical carrier order)
+    const int32_t* active;                       // [S] the step decoded a frame
+    const int64_t* prs; const int64_t* buf_start;   // [S] the phase reference symbol, relative to the buffer; the buffer's first sample
+    void* res;                                   // [S] dabb_combine_result (tap 12): noise in, members and mask out
+    int8_t* soft; int64_t soft_stride;           // the step's softbits: the leaders' rows are overwritten
+    int weighted;                                // DABB_DEMAP_WEIGHTED
+};
+void launch_combine(const CombParams& p, cudaStream_t st);
 
 // ---- TII analysis (tii.cu, tii_core.cuh) ----
 struct TiiParams {

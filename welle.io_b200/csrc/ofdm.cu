@@ -375,7 +375,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
     DemodSmem& sm = *reinterpret_cast<DemodSmem*>(smraw);
     const int t = threadIdx.x;
     // ---- once per CTA
-    if (t == 0) { mbar_init(&sm.full, 1); if (!TAP) mbar_init(&sm.half1, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+    if (t == 0) { mbar_init(&sm.full, 1); mbar_init(&sm.half1, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
     if (t < TwLayout::C4) sm.tw[t] = tb.tw_fwd[t];
     const float2* tw_c5 = tb.tw_fwd + TwLayout::C5;
     const XIdx xi = make_xidx(t);
@@ -427,7 +427,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
     };
     // what each symbol of the frame needs (CTA-uniform): transformed when it is the phase reference symbol, demapped, or the reference of
     // a demapped symbol; light otherwise.  No mask: every symbol is transformed and demapped.
-    if (!TAP && t < NSYM) {
+    if (t < NSYM) {
         const uint32_t* m = p.symmask ? p.symmask + (int64_t)f * OFDM_MASK_WORDS : nullptr;
         const bool dm = !m || ((m[t >> 5] >> (t & 31)) & 1u), dm1 = !m || (t + 1 < NSYM && ((m[(t + 1) >> 5] >> ((t + 1) & 31)) & 1u));
         sm.kind[t] = (t > 0 && dm) ? SYM_DEMAP : ((t == 0 || dm1) ? SYM_FFT : SYM_LIGHT);
@@ -441,7 +441,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
         const int k = t & 15;
         sm.rtab[t >> 4][k] = osc_fast(mod_rate64(-(int64_t)(128 * (k >> 3) + 256 * (k & 7)) * n.ph));
     }
-    if (FASTNCO || !TAP) __syncthreads();
+    __syncthreads();
     // CLOCK: the frame's ppm (CTA-uniform); 0 leaves r1 untouched.  Carrier k = t + 128 j of this thread is derotated by P * Q[j]
     // (dabb_clock::phasor): P in registers, Q[1..6] in shared memory, written here and first read after barrier (1) of the first symbol
     float2 ckp = make_float2(1.f, 0.f);
@@ -462,11 +462,25 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
         return dabb_clock::cmul(ckp, j < 0 ? make_float2(q.x, -q.y) : q);
     };
 
+    // TAP: where symbol l's r1 goes (CTA-uniform), nullptr for nowhere.  Without r1_row, row f * 75 + l - 1 (the constellation tap);
+    // with it, row r1_row[f] (< 0: the frame stores nothing) plus the symbol's column: l - 1 without r1_lmask, else its rank among the
+    // symbols r1_lmask[f] marks (a diversity group's leader's symbols, combine.cu), nothing for the symbols it does not mark
+    auto r1_dst = [&](int l) -> float2* {
+        if (!p.r1_row) return p.r1 + ((int64_t)f * 75 + (l - 1)) * KC;
+        const int32_t b = p.r1_row[f];
+        if (b < 0) return nullptr;
+        if (!p.r1_lmask) return p.r1 + ((int64_t)b + (l - 1)) * KC;
+        const uint32_t* m = p.r1_lmask + (int64_t)f * OFDM_MASK_WORDS;
+        if (!((m[l >> 5] >> (l & 31)) & 1u)) return nullptr;
+        int c = __popc(m[l >> 5] & ((1u << (l & 31)) - 1u));
+        for (int w = 0; w < (l >> 5); w++) c += __popc(m[w]);
+        return p.r1 + ((int64_t)b + c) * KC;
+    };
+
     // Staging: inbuf holds one transformed symbol or two light ones.  Symbols are copied in order, each as soon as its space is free
     // (a transformed one needs both halves); light symbols alternate between the halves.  The reference symbol l_first - 1 of a later
     // item is staged only when it is transformed: a light one contributes nothing to this item.
-    // (the TAP instances always run without a mask: every symbol is transformed)
-    auto kind_of = [&](int l) -> int { return TAP ? (l ? SYM_DEMAP : SYM_FFT) : sm.kind[l]; };
+    auto kind_of = [&](int l) -> int { return sm.kind[l]; };
     const int l_begin = (l_first > 1 && kind_of(l_first - 1) == SYM_LIGHT) ? l_first : l_first - 1;
     int nxt = l_begin;                    // next symbol to copy
     int used = 0, ih = 0, ch = 0;         // halves in use; half of the next light copy, of the next light symbol to consume
@@ -520,6 +534,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
                 // DABB_DEMAP_WEIGHTED: r1 of every owned bin into v[] (its spectrum moves to prev[]), the symbol's geometric-mean carrier
                 // level G from one block reduction, then the demap against max(l1, G) (ofdm_core.cuh: level_acc, level_gmean)
                 LevelSum ls{0, 0.f};
+                float2* const r1d = TAP ? r1_dst(l) : nullptr;
 #pragma unroll
                 for (int s = 0; s < NSLOT; s++) {
                     const float2 X = v[slot_c(s)];
@@ -536,10 +551,11 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
                     int8_t sre, sim;
                     demap_weighted(r1, G, rG, sre, sim);
                     sm.sbuf[sidx[s]] = (uint16_t)((uint8_t)sre | ((uint16_t)(uint8_t)sim << 8));
-                    if (TAP) { const int c0 = tb.invperm[t + 128 * slot_c(s)]; if (c0 >= 0) p.r1[((int64_t)f * 75 + (l - 1)) * KC + c0] = r1; }
+                    if (TAP && r1d) { const int c0 = tb.invperm[t + 128 * slot_c(s)]; if (c0 >= 0) r1d[c0] = r1; }
                 }
             } else {
             // demap owned bins against the previous symbol, scatter softbits into logical order (branch free)
+            float2* const r1d = TAP ? r1_dst(l) : nullptr;
 #pragma unroll
             for (int s = 0; s < NSLOT; s++) {
                 const float2 X = v[slot_c(s)];
@@ -550,7 +566,7 @@ ofdm_demod_kernel(DevTables tb, OfdmParams p)
                     demap_r1(r1, sre, sim);
                 } else demap_one<EXACT>(X, prev[s], sre, sim, r1);
                 sm.sbuf[sidx[s]] = (uint16_t)((uint8_t)sre | ((uint16_t)(uint8_t)sim << 8));
-                if (TAP) { const int c0 = tb.invperm[t + 128 * slot_c(s)]; if (c0 >= 0) p.r1[((int64_t)f * 75 + (l - 1)) * KC + c0] = r1; }
+                if (TAP && r1d) { const int c0 = tb.invperm[t + 128 * slot_c(s)]; if (c0 >= 0) r1d[c0] = r1; }
                 prev[s] = X;
             }
             }

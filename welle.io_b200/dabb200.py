@@ -81,6 +81,10 @@ assert BER_DTYPE.itemsize == 80
 # dabb_clock_result: one stream's sample-clock estimate of one step (tap 11)
 CLOCK_DTYPE = np.dtype([("ppm", "<f4"), ("applied_ppm", "<f4"), ("frames", "<i4"), ("reserved", "<i4")])
 assert CLOCK_DTYPE.itemsize == 16
+# dabb_combine_result: one stream's diversity combination of one step (tap 12)
+MAX_BRANCHES = 8
+COMBINE_DTYPE = np.dtype([("members", "<i4"), ("mask", "<u4"), ("noise", "<f4"), ("reserved", "<i4")])
+assert COMBINE_DTYPE.itemsize == 16
 
 
 class IO(C.Structure):
@@ -90,7 +94,7 @@ class IO(C.Structure):
 
 
 EXPORTS = ["dabb_create", "dabb_destroy", "dabb_last_error", "dabb_abi_version", "dabb_stream_reset", "dabb_set_options", "dabb_get_info", "dabb_select_subchannel",
-           "dabb_remove_subchannel", "dabb_process", "dabb_process_async", "dabb_sync", "dabb_join_lanes", "dabb_submit", "dabb_collect", "dabb_cuda_stream", "dabb_kernel_launches",
+           "dabb_remove_subchannel", "dabb_set_combining", "dabb_process", "dabb_process_async", "dabb_sync", "dabb_join_lanes", "dabb_submit", "dabb_collect", "dabb_cuda_stream", "dabb_kernel_launches",
            "dabb_read_tap", "dabb_profile", "dabb_profile_read", "dabb_ofdm_demod", "dabb_ofdm_demod_ex", "dabb_find_index", "dabb_find_index_ex", "dabb_coarse_estimate", "dabb_viterbi", "dabb_fic_decode", "dabb_msc_decode",
            "dabb_rs_superframes", "dabb_dev_alloc", "dabb_dev_free", "dabb_memcpy_h2d", "dabb_memcpy_d2h",
            "dabb_chan_create", "dabb_chan_destroy", "dabb_chan_input_range", "dabb_channelize", "dabb_survey", "dabb_survey_candidates"]
@@ -286,6 +290,16 @@ class Context:
         """streams [first, first + count) stop decoding `slot`; the slot's other streams decode on unchanged"""
         self._ck(self.lib.dabb_remove_subchannel(self.h, first, self.n_streams if count is None else count, slot))
 
+    def set_combining(self, leader=None):
+        """diversity reception (dabb_set_combining): leader[s] == s for a stream that is alone or leads a group, else the stream whose
+        group s joins (at most MAX_BRANCHES members per group, leader included); None dissolves every group.  Each leader's softbits
+        become the demap of its group's noise-weighted differential products; every other member decodes on as it would alone."""
+        if leader is None:
+            self._ck(self.lib.dabb_set_combining(self.h, None, self.n_streams))
+            return
+        t = np.ascontiguousarray(leader, np.int32)
+        self._ck(self.lib.dabb_set_combining(self.h, _vp(t), C.c_int32(t.size)))
+
     def process(self, iq, stride, buf_start, buf_len, iq_is_host=False, msc_stride=0, sf_stride=0, want=("results", "fibs"), iq_format=0):
         S = self.n_streams
         bs = np.ascontiguousarray(buf_start, np.int64)
@@ -372,7 +386,8 @@ class Context:
         """0 softbits, 1 CIR, 2 constellation points (75 x 16 per stream), 3 null symbol (2656 samples, NCO applied),
         4 TII spectra (PRS, null symbol), 5 frame results, 6 FIBs, 7 logical frames [S, MAX_SUBCH, 4, stride] and 8 superframes
         [S, MAX_SUBCH, stride] of the last step (also after process_async), 9 TII measurements (TII_DTYPE per stream), 10 channel bit
-        errors (BER_DTYPE per stream), 11 sample-clock estimates (CLOCK_DTYPE per stream)"""
+        errors (BER_DTYPE per stream), 11 sample-clock estimates (CLOCK_DTYPE per stream), 12 diversity combinations (COMBINE_DTYPE per
+        stream)"""
         if what == 7:
             out = np.zeros((self.n_streams, MAX_SUBCH, 4, stride), np.uint8)
         elif what == 8:
@@ -395,6 +410,8 @@ class Context:
             out = np.zeros(self.n_streams, BER_DTYPE)
         elif what == 11:
             out = np.zeros(self.n_streams, CLOCK_DTYPE)
+        elif what == 12:
+            out = np.zeros(self.n_streams, COMBINE_DTYPE)
         else:
             out = np.zeros((self.n_streams, TU), np.float32)
         self._ck(self.lib.dabb_read_tap(self.h, what, _vp(out), C.c_size_t(out.nbytes)))

@@ -3,7 +3,7 @@
  * wideband file, --rate), on one GPU.
  *
  *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock]
- *                [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file1 [file2 ...]
+ *                [--diversity N] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file1 [file2 ...]
  *
  * What `welle-cli -f FILE -D` does for one recording (welle-cli.cpp:215-235,612-707: dump the FIC, tune to the first audio
  * service, dump its logical frames) done for all files in lock-step: every iteration hands each stream's next window of samples
@@ -28,6 +28,12 @@
  * --offset auto survey and confirmation contexts included: each stream estimates its recording's sample-clock error from its frame
  * timing and the demodulator removes the phase ramp it puts on the softbits.  Every decoded frame adds one line "ppm applied_ppm frames"
  * (tap 11) to DIR/<name>.clk.
+ *
+ * --diversity N: consecutive runs of N files are the antennas of one capture (one coherent receiver's files: same rate, same first
+ * sample); the first file of each run leads its group (dabb_set_combining) and decodes from the noise-weighted sum of the group's
+ * differential products.  Every file keeps its outputs as without the option (the leader's are those of the combination, the others'
+ * their own antenna's), and every decoded frame of a leader adds one line "members mask noise" (tap 12) to DIR/<name>.div.  1 <= N <=
+ * DABB_MAX_BRANCHES, the file count a multiple of N; not with --rate.
  *
  * --rate HZ --offset HZ[,HZ...]: every file is a wideband recording at HZ samples/s (any rate dabb_chan_create accepts) and every offset
  * (Hz from the tuned frequency, may be negative) is one stream of the batch, decoded by a channelizer of the same context (dabb_chan_*):
@@ -75,6 +81,7 @@ namespace {
 
 struct Stream {
     std::string path, name; FILE* in = nullptr; FILE* fic = nullptr; FILE* msc = nullptr; FILE* rs = nullptr; FILE* tii = nullptr; FILE* ber = nullptr; FILE* clk = nullptr;
+    FILE* div = nullptr;                                          /* --diversity: a group leader's combinations */
     int64_t buf_start = 0, have = 0, pos = 0, acq_need = 0;      /* logical sample indices; `have` samples are buffered from buf_start */
     bool tracking = false, eof = false, done = false;
     std::unique_ptr<dabb_host::FigDb> db{new dabb_host::FigDb()};
@@ -96,6 +103,7 @@ struct Wide {
 struct Outputs {
     std::vector<dabb_frame_result> res; std::vector<uint8_t> fibs, msc, sf; std::vector<dabb_tii_result> tres; std::vector<dabb_ber_result> bres;
     std::vector<dabb_clock_result> cres;        /* tap 11, read after every step when not empty (--clock) */
+    std::vector<dabb_combine_result> dres;      /* tap 12, read after every step when not empty (--diversity) */
 };
 
 /* the receiver position after one step's result r of stream s: 0 = the stream ended, 1 = no frame decoded, 2 = a frame was decoded */
@@ -132,6 +140,10 @@ bool handle_result(dabb_ctx* ctx, Stream& z, int s, const Outputs& o, bool tii, 
     if (z.clk) {
         const dabb_clock_result& c = o.cres[(size_t)s];
         fprintf(z.clk, "%.4f %.4f %d\n", c.ppm, c.applied_ppm, c.frames);
+    }
+    if (z.div) {
+        const dabb_combine_result& d = o.dres[(size_t)s];
+        fprintf(z.div, "%d %u %.6e\n", d.members, d.mask, d.noise);
     }
     for (int f = 0; f < 12; f++) {
         const uint8_t* fb = o.fibs.data() + ((size_t)s * 12 + (size_t)f) * 32;
@@ -205,6 +217,7 @@ bool step(dabb_ctx* ctx, Outputs& o, std::vector<int64_t>& buf_start, const floa
     if (tii && dabb_read_tap(ctx, 9, o.tres.data(), o.tres.size() * sizeof(dabb_tii_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     if (ber && dabb_read_tap(ctx, 10, o.bres.data(), o.bres.size() * sizeof(dabb_ber_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     if (!o.cres.empty() && dabb_read_tap(ctx, 11, o.cres.data(), o.cres.size() * sizeof(dabb_clock_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
+    if (!o.dres.empty() && dabb_read_tap(ctx, 12, o.dres.data(), o.dres.size() * sizeof(dabb_combine_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     return true;
 }
 
@@ -473,7 +486,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
 int main(int argc, char** argv)
 {
     int fmt = DABB_IQ_CF32, device = 0, soft = DABB_DEMAP_REFERENCE, clock = DABB_CLOCK_OFF; bool coarse = false, tii = false, ber = false; std::string out;
-    int64_t rate = 0; std::vector<int64_t> offsets; bool scan_only = false, auto_offsets = false;
+    int64_t rate = 0; std::vector<int64_t> offsets; bool scan_only = false, auto_offsets = false; int diversity = 0; bool diversity_set = false;
     std::vector<std::string> files;
     for (int i = 1; i < argc; i++) {
         const std::string a = argv[i];
@@ -488,6 +501,7 @@ int main(int argc, char** argv)
         else if (a == "--tii") tii = true;
         else if (a == "--ber") ber = true;
         else if (a == "--clock") clock = DABB_CLOCK_TRACK;
+        else if (a == "--diversity" && i + 1 < argc) { diversity = atoi(argv[++i]); diversity_set = true; }
         else if (a == "--soft" && i + 1 < argc) {
             const std::string m = argv[++i];
             soft = m == "reference" ? DABB_DEMAP_REFERENCE : m == "weighted" ? DABB_DEMAP_WEIGHTED : -1;
@@ -508,7 +522,11 @@ int main(int argc, char** argv)
     }
     if (out.empty() || files.empty() || (rate > 0) != ((int)!offsets.empty() + (int)scan_only + (int)auto_offsets == 1)
         || (rate <= 0 && (scan_only || auto_offsets))) {
-        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
+        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock] [--diversity N] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
+        return 2;
+    }
+    if (diversity_set && (rate > 0 || diversity < 1 || diversity > DABB_MAX_BRANCHES || files.size() % (size_t)diversity)) {
+        fprintf(stderr, "batch_decode: --diversity N needs 1 <= N <= %d, a file count that is a multiple of N, and no --rate\n", DABB_MAX_BRANCHES);
         return 2;
     }
     const bool wide = rate > 0;
@@ -555,6 +573,11 @@ int main(int argc, char** argv)
         op.disable_coarse = cfg.disable_coarse; op.decode_tii = tii; op.count_bit_errors = ber; op.soft_demap = soft; op.sample_clock = clock;
         if (dabb_set_options(ctx, &op) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
     }
+    if (diversity > 1) {          /* the antennas of one capture: the first file of each run of `diversity` leads */
+        std::vector<int32_t> leader((size_t)S);
+        for (int s = 0; s < S; s++) leader[(size_t)s] = s - s % diversity;
+        if (dabb_set_combining(ctx, leader.data(), S) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
+    }
 
     std::vector<Stream> st((size_t)S);
     std::vector<Wide> wf(wide ? files.size() : 0);
@@ -576,14 +599,16 @@ int main(int argc, char** argv)
         if (tii) z.tii = fopen((out + "/" + z.name + ".tii").c_str(), "w");
         if (ber) z.ber = fopen((out + "/" + z.name + ".ber").c_str(), "w");
         if (clock) z.clk = fopen((out + "/" + z.name + ".clk").c_str(), "w");
-        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii) || (ber && !z.ber) || (clock && !z.clk)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
+        const bool leads = diversity > 1 && s % diversity == 0;
+        if (leads) z.div = fopen((out + "/" + z.name + ".div").c_str(), "w");
+        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii) || (ber && !z.ber) || (clock && !z.clk) || (leads && !z.div)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
         z.acq_need = 3 * TF;
     }
     dabb_stream_reset(ctx, 0, S, 0);
 
     Outputs o;
     o.res.resize((size_t)S); o.fibs.resize((size_t)S * 12 * 32); o.msc.resize((size_t)S * DABB_MAX_SUBCH * 4 * 1152); o.sf.resize((size_t)S * DABB_MAX_SUBCH * 5760);
-    o.tres.resize(tii ? (size_t)S : 0); o.bres.resize(ber ? (size_t)S : 0); o.cres.resize(clock ? (size_t)S : 0);
+    o.tres.resize(tii ? (size_t)S : 0); o.bres.resize(ber ? (size_t)S : 0); o.cres.resize(clock ? (size_t)S : 0); o.dres.resize(diversity > 1 ? (size_t)S : 0);
     std::vector<int64_t> buf_start((size_t)S);
 
     int active = S;
@@ -641,7 +666,7 @@ int main(int argc, char** argv)
     for (auto& z : st) {
         printf("%s frames=%ld fibs=%ld fib_crc_ok=%ld service=0x%X bitrate=%d logical_frames=%ld\n", z.name.c_str(), z.frames, z.fibs, z.fibs_ok, z.sid, z.bitrate, z.logical);
         if (z.in) fclose(z.in);
-        fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii); if (z.ber) fclose(z.ber); if (z.clk) fclose(z.clk);
+        fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii); if (z.ber) fclose(z.ber); if (z.clk) fclose(z.clk); if (z.div) fclose(z.div);
     }
     dabb_destroy(ctx);
     return 0;
