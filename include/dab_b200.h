@@ -143,7 +143,7 @@ typedef struct {
  * group, any other value is the stream whose group s joins.  Every entry must satisfy leader[leader[s]] == leader[s], and a group has at
  * most DABB_MAX_BRANCHES members, its leader included; NULL dissolves every group.  A malformed table (an index out of range, a chain, an
  * oversized group, a wrong n) returns DABB_E_ARG and changes nothing.  Like a select call, the function waits for outstanding work and
- * takes effect from the next step; dabb_stream_reset does not change the grouping.  The members of a group must share one logical sample
+ * takes effect from the next step (tap 0 of the last step keeps that step's combination); dabb_stream_reset does not change the grouping.  The members of a group must share one logical sample
  * axis (buf_start), as the files of one coherent capture do.
  * In a step where leader L decodes a frame (DABB_FRAME_DECODED):
  *   A_x = buf_start[x] + the start of x's phase reference symbol in its buffer, the symbol's absolute position;

@@ -1,6 +1,6 @@
 """numpy restatement of diversity combining (dabb_set_combining, include/dab_b200.h), TEST TOOLING.
 
-noise(y): N = mean |y|^2 of a null symbol in float64.  select(): the contributor rule.  combined(): R = sum over the contributors of
+noise(y): N = mean |y|^2 of a null symbol in float64, noise_f32(y) the same in the library's float32 order.  select(): the contributor rule.  combined(): R = sum over the contributors of
 r1_b / N_b in float64 (ascending stream order), and soft(): the reference or weighted demap of R in float64 (softbit 0 where the value is
 not finite).  combined_f32() is the same sum in float32 with every operation rounded in the library's order, so that the order of the
 contributors can be checked bit for bit."""
@@ -16,6 +16,25 @@ def noise(y):
     y = np.asarray(y).astype(np.complex128)
     with np.errstate(all="ignore"):
         return np.mean(y.real ** 2 + y.imag ** 2, axis=-1)
+
+
+def noise_f32(y):
+    """N of null symbols y [..., TNULL] in the library's float32 order: the partial sums of Re^2 + Im^2 over i = t mod 256 in ascending
+    i, then the 256 partials in order, divided by TNULL (each operation rounded): bit for bit the library's value"""
+    y = np.asarray(y).astype(np.complex64)
+    lead = y.shape[:-1]
+    re, im = y.real.astype(np.float32), y.imag.astype(np.float32)
+    with np.errstate(all="ignore"):
+        p = ((re * re).astype(np.float32) + (im * im).astype(np.float32)).astype(np.float32)
+        pad = np.zeros(lead + (256 * 11,), np.float32)
+        pad[..., :TNULL] = p
+        part = np.zeros(lead + (256,), np.float32)
+        for k in range(11):
+            part = (part + pad[..., 256 * k:256 * k + 256]).astype(np.float32)
+        tot = np.zeros(lead, np.float32)
+        for t in range(256):
+            tot = (tot + part[..., t]).astype(np.float32)
+        return (tot / np.float32(TNULL)).astype(np.float32)
 
 
 def noise_ok(n):
@@ -55,7 +74,9 @@ def combined_f32(r1, nz, mask, order=None):
             with np.errstate(all="ignore"):
                 re = (re + (r[i].real.astype(np.float32) / n).astype(np.float32)).astype(np.float32)
                 im = (im + (r[i].imag.astype(np.float32) / n).astype(np.float32)).astype(np.float32)
-    return (re + 1j * im.astype(np.complex64)).astype(np.complex64)
+    out = np.empty(re.shape, np.complex64)                # (re + 1j * im would turn an infinite im into a NaN re)
+    out.real, out.imag = re, im
+    return out
 
 
 def exact(R, weighted):

@@ -57,16 +57,7 @@ def test_noise(emul):
     want = combineref.noise(y.astype(np.complex64))
     assert np.all(np.abs(got - want) <= 1e-5 * want), (got, want)
     # the fixed order: partial sums of i = t mod 256 in ascending i, then the partials in order (float32, each operation rounded)
-    y32 = y.astype(np.complex64)
-    p = (y32.real * y32.real + y32.imag * y32.imag).astype(np.float32)
-    pad = np.zeros((6, 256 * 11), np.float32); pad[:, :combineref.TNULL] = p
-    part = np.zeros((6, 256), np.float32)
-    for k in range(11):
-        part = (part + pad[:, 256 * k:256 * k + 256]).astype(np.float32)
-    tot = np.zeros(6, np.float32)
-    for t in range(256):
-        tot = (tot + part[:, t]).astype(np.float32)
-    assert np.array_equal(got, (tot / np.float32(combineref.TNULL)).astype(np.float32))
+    assert np.array_equal(got, combineref.noise_f32(y))
     z = np.zeros((3, combineref.TNULL), np.complex64)
     z[1, 7] = np.inf; z[2, 100] = np.nan
     g = host_noise(emul, z)
@@ -147,3 +138,52 @@ def test_unusable_noise(emul, weighted):
     # the leader's own noise unusable: it decodes alone
     nz = np.array([np.nan, 1.0, 1.0, 1.0], np.float32)
     assert emul.emul_combine_select(4, 0, _p(np.ones(4, np.int32)), _p(np.zeros(4, np.int64)), _p(nz)) == 1
+
+
+FLT_MIN, SUBNORMAL = np.float32(2.0 ** -126), np.float32(2.0 ** -140)
+
+
+def _edge_cases(rng):
+    """(name, r1 [3, K], N [3], contributor mask) at the scale edges of the combination"""
+    r1 = members(rng, 3)
+    out = []
+    for tiny in (FLT_MIN, SUBNORMAL):                         # r1 / N overflows to +-inf on most carriers, stays finite on the rest
+        out.append((f"N {tiny:g}", r1, np.array([0.5, tiny, 2.0], np.float32), 0b111))
+    r = r1.copy(); r[2] = -r[0]                               # +inf and -inf terms of two members: NaN in R
+    out.append(("opposite infinities", r, np.array([SUBNORMAL, 1.0, SUBNORMAL], np.float32), 0b111))
+    r = r1.copy(); r[1] = -r[0]; r[1, 1::2] *= 0.5            # R exactly 0 on every other carrier (and -0 in a component)
+    r[0, ::5] = r[0, ::5].real                                # some components 0 in both members
+    r[1, ::5] = -r[0, ::5]
+    out.append(("R = 0", r, np.array([0.75, 0.75, 1.0], np.float32), 0b011))
+    r = r1.copy()                                             # inf and NaN in one member's r1
+    r[1, ::7] = np.inf; r[1, 3::7] = complex(np.nan, 1.0); r[1, 5::11] = complex(-np.inf, np.inf); r[1, 6::13] = complex(2.0, np.nan)
+    out.append(("inf / NaN in r1", r, np.array([0.5, 1.5, 2.0], np.float32), 0b111))
+    return out
+
+
+@pytest.mark.parametrize("weighted", [False, True])
+def test_scale_edges(emul, weighted):
+    """the combined softbits where R leaves the finite range: a valid but tiny N (FLT_MIN, subnormal) whose quotients overflow to
+    +-inf, infinite terms of opposite signs (NaN), R exactly 0, inf and NaN in one member's r1.  The reference demap is bit for bit
+    softref.soft_reference_f32 of the float32 sum in ascending stream order; a carrier whose R is not finite, or 0, gets softbit 0 (DESIGN
+    5: NaN gives 0); a symbol with a level that is not finite has G = 0, so the weighted demap is the reference demap there, and elsewhere
+    it is the restatement of tests/softref.py.  (The host build's reciprocal is the IEEE quotient; for a combined level l1 >= 2^126 the
+    device's flushes to 0, the demap's documented range, DESIGN 5.)"""
+    rng = np.random.default_rng(0xC0B6 + int(weighted))
+    for name, r1, nz, mask in _edge_cases(rng):
+        assert emul.emul_combine_select(3, 0, _p(np.ones(3, np.int32)), _p(np.zeros(3, np.int64)), _p(nz)) == 0b111, name   # tiny N is valid
+        got = host_symbol(emul, r1, nz, mask, weighted)
+        R = combineref.combined_f32(r1, nz, mask)
+        ref = softref.soft_reference_f32(R)
+        re_bad = ~np.isfinite(R.real) | ~np.isfinite(R.imag) | (R == 0)
+        assert not got[:K][re_bad].any() and not got[K:][re_bad].any(), name
+        if name != "R = 0":
+            assert re_bad.sum() > K // 8, (name, int(re_bad.sum()))
+        else:
+            assert (R == 0).sum() >= K // 2 and got[:K].any(), name
+        if not weighted:
+            assert np.array_equal(got, ref), (name, int((got != ref).sum()))
+        elif not np.isfinite(softref.levels(R)[2]).all():
+            assert np.array_equal(got, host_symbol(emul, r1, nz, mask, False)) and np.array_equal(got, ref), name
+        else:
+            softref.check(R, got)

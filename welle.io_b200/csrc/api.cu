@@ -160,12 +160,15 @@ struct dabb_ctx {
     // diversity combining (dabb_set_combining, combine.cu), all empty until a group of two or more forms (comb_on): the leader table; per
     // group its members and their r1 rows (d_comb_groups) and the (group, symbol) items of combine_kernel (d_comb_items); per stream its
     // group or -1 (d_comb_gid).  Without keep_taps the OFDM kernel stores the grouped streams' r1 of their leader's symbols in d_comb_r1
-    // (row d_comb_row[s], the symbols d_comb_lmask[s] marks); with it combine_kernel reads tap 2's d_r1.  d_comb_groups_full /
-    // d_comb_row_full: the rows of every symbol, for the tap-0 repeat.  d_comb_res: tap 12, kept once allocated; comb_op: the last
-    // step's combine launch
+    // (row d_comb_row[s], the symbols d_comb_lmask[s] marks); with it combine_kernel reads tap 2's d_r1.  d_comb_res: tap 12, kept once
+    // allocated.  The tap-0 repeat of the last step: comb_op, that step's combine launch (n_items 0: it had no group), and the grouping it
+    // ran with, the rows of every symbol (d_comb_groups_full, d_comb_row_full, comb_n_groups groups of comb_n_grouped streams in all).  A
+    // regroup stages the new grouping's (the *_next members, comb_staged) and the next step takes them over, so that tap 0 of the step
+    // before the regroup stays combined
     std::vector<int32_t> h_leader; bool comb_on = false; int comb_n_groups = 0, comb_n_items = 0, comb_n_grouped = 0;
     DevBuf<CombGroup> d_comb_groups, d_comb_groups_full; DevBuf<CombItem> d_comb_items; DevBuf<int32_t> d_comb_gid, d_comb_row, d_comb_row_full;
     DevBuf<uint32_t> d_comb_lmask; DevBuf<float2> d_comb_r1; DevBuf<dabb_combine_result> d_comb_res; CombParams comb_op{};
+    DevBuf<CombGroup> d_comb_groups_next; DevBuf<int32_t> d_comb_row_next; int comb_next_groups = 0, comb_next_grouped = 0; bool comb_staged = false;
 };
 
 namespace {
@@ -697,8 +700,9 @@ template <typename T> int upload(dabb_ctx* ctx, DevBuf<T>& b, const std::vector<
 
 // the tables of diversity combining from h_leader and the leaders' symbol masks (the caller has run sync_all).  Each group of two or more
 // streams combines the data symbols its leader's decoders read (every symbol with keep_taps); without keep_taps its members' r1 rows of
-// those symbols lie one after the other in d_comb_r1.  `regroup`: the grouping itself changed, so the tap-0 repeat's rows are rebuilt too
-// and the last step's combination is not repeated.  No group: every table is freed (tap 12's records stay).
+// those symbols lie one after the other in d_comb_r1.  `regroup`: the grouping itself changed, so the rows of every symbol are staged for
+// the tap-0 repeat of the next step; the last step's stay for its own repeat.  No group: every table the next step would read is freed
+// (tap 12's records stay).
 int rebuild_comb(dabb_ctx* ctx, bool regroup)
 {
     const int S = ctx->S, W = OFDM_MASK_WORDS;
@@ -735,11 +739,14 @@ int rebuild_comb(dabb_ctx* ctx, bool regroup)
         groups.push_back(g); full.push_back(gf);
     }
     ctx->comb_on = !groups.empty();
-    if (regroup) ctx->comb_op = CombParams{};
+    if (regroup) {
+        ctx->d_comb_groups_next.reset(); ctx->d_comb_row_next.reset();
+        ctx->comb_next_groups = ctx->comb_next_grouped = 0; ctx->comb_staged = true;
+    }
     if (!ctx->comb_on) {
-        ctx->d_comb_groups.reset(); ctx->d_comb_groups_full.reset(); ctx->d_comb_items.reset(); ctx->d_comb_gid.reset(); ctx->d_comb_row.reset();
-        ctx->d_comb_row_full.reset(); ctx->d_comb_lmask.reset(); ctx->d_comb_r1.reset();
-        ctx->comb_n_groups = ctx->comb_n_items = ctx->comb_n_grouped = 0;
+        ctx->d_comb_groups.reset(); ctx->d_comb_items.reset(); ctx->d_comb_gid.reset(); ctx->d_comb_row.reset();
+        ctx->d_comb_lmask.reset(); ctx->d_comb_r1.reset();
+        ctx->comb_n_items = 0;
         return DABB_OK;
     }
     int rc;
@@ -747,10 +754,13 @@ int rebuild_comb(dabb_ctx* ctx, bool regroup)
     if (!taps) {
         if ((rc = upload(ctx, ctx->d_comb_row, row)) || (rc = upload(ctx, ctx->d_comb_lmask, lmask))) return rc;
         if ((size_t)rows * KC > ctx->d_comb_r1.size() || (size_t)rows * KC * 2 < ctx->d_comb_r1.size()) { ctx->d_comb_r1.reset(); if ((rc = alloc(ctx, ctx->d_comb_r1, (size_t)rows * KC))) return rc; }
-        if (regroup && ((rc = upload(ctx, ctx->d_comb_groups_full, full)) || (rc = upload(ctx, ctx->d_comb_row_full, row_full)))) return rc;
+        if (regroup) {
+            if ((rc = upload(ctx, ctx->d_comb_groups_next, full)) || (rc = upload(ctx, ctx->d_comb_row_next, row_full))) return rc;
+            ctx->comb_next_groups = (int)groups.size(); ctx->comb_next_grouped = rank;
+        }
     }
     CK(cudaStreamSynchronize(ctx->stream));
-    ctx->comb_n_groups = (int)groups.size(); ctx->comb_n_items = (int)items.size(); ctx->comb_n_grouped = rank;
+    ctx->comb_n_items = (int)items.size();
     return DABB_OK;
 }
 
@@ -1182,7 +1192,13 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         }
     }
     if (!ctx->decode_tii && ctx->d_tii_res) CK(cudaMemsetAsync(ctx->d_tii_res, 0, sizeof(dabb_tii_result) * S, A));     // tap 9: nothing analysed in this step
-    // diversity combining: the members' noise powers, then the leaders' softbits from their groups' products
+    // diversity combining: the members' noise powers, then the leaders' softbits from their groups' products.  The tap-0 repeat of this
+    // step uses the grouping staged by a regroup since the last step
+    if (ctx->comb_staged) {
+        ctx->d_comb_groups_full = std::move(ctx->d_comb_groups_next); ctx->d_comb_row_full = std::move(ctx->d_comb_row_next);
+        ctx->comb_n_groups = ctx->comb_next_groups; ctx->comb_n_grouped = ctx->comb_next_grouped; ctx->comb_staged = false;
+    }
+    ctx->comb_op = CombParams{};
     if (ctx->comb_on) {
         null_power_kernel<<<S, dabb_comb::NULL_THREADS, 0, A>>>(scr, ctx->d_comb_gid, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, ctx->d_comb_res);
         if ((rc = check_launch(ctx, "null_power_kernel"))) return rc;
