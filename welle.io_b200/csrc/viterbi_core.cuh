@@ -1,6 +1,5 @@
 // viterbi_core.cuh — per-thread K=7 rate-1/4 Viterbi add-compare-select, one codeword per thread, all 64 path
-// metrics in 32 registers as packed signed 16-bit pairs (VIMNMX.S16x2 with two predicate outputs + VIADD.16x2 on
-// sm_90a).
+// metrics in 32 registers as packed signed 16-bit pairs (VIADDMNMX.S16x2 on sm_90a).
 //
 // Semantics reproduced from the reference (backend/viterbi.cpp): polynomials 0155 0117 0123 0155 (:35-36); branch
 // metric = sum_k (sym_k or 255 - sym_k) (:248-261); new[2i] = min(old[i] + m, old[i+32] + 1020 - m),
@@ -11,7 +10,7 @@
 //
 // Register layout.  Layout L_b pairs, in one 32-bit register, the two states that differ in bit b (low half: bit
 // b = 0).  An ACS step maps L_b -> L_{b+1} with plain SIMD (two butterflies per pair of registers, no data movement);
-// L_5 pairs butterfly partners, so that step duplicates halves with PRMT and lands in L_0.  Six consecutive steps
+// L_5 pairs butterfly partners, so that step swaps halves with PRMT and lands in L_0.  Six consecutive steps
 // (nsteps = nbits + 6 is always a multiple of 6) are unrolled with compile-time register indices.
 #pragma once
 #include <stdint.h>
@@ -45,20 +44,12 @@ VIT_HD uint32_t vibmin16(uint32_t a, uint32_t b, bool& ph, bool& pl)
     return (uint32_t)(uint16_t)(pl ? al : bl) | ((uint32_t)(uint16_t)(ph ? ah : bh) << 16);
 #endif
 }
-VIT_HD uint32_t dup_lo(uint32_t r)
+VIT_HD uint32_t swap16(uint32_t r)
 {
 #if defined(__CUDA_ARCH__)
-    return __byte_perm(r, 0, 0x1010);
+    return __byte_perm(r, 0, 0x1032);
 #else
-    return (r & 0xFFFF) | (r << 16);
-#endif
-}
-VIT_HD uint32_t dup_hi(uint32_t r)
-{
-#if defined(__CUDA_ARCH__)
-    return __byte_perm(r, 0, 0x3232);
-#else
-    return (r >> 16) | (r & 0xFFFF0000u);
+    return (r >> 16) | (r << 16);
 #endif
 }
 VIT_HD uint32_t vminu16x2(uint32_t a, uint32_t b)
@@ -78,6 +69,16 @@ VIT_HD uint32_t vmin16(uint32_t a, uint32_t b)
     uint32_t r; asm("min.s16x2 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(b)); return r;
 #else
     bool ph, pl; return vibmin16(a, b, ph, pl);
+#endif
+}
+// per-half min(a + b, c), the sums wrapping within their half (SASS: VIADDMNMX.S16x2)
+VIT_HD uint32_t vaddmin16(uint32_t a, uint32_t b, uint32_t c)
+{
+#if defined(__CUDA_ARCH__)
+    return __viaddmin_s16x2(a, b, c);
+#else
+    const uint32_t s = ((a + b) & 0xFFFFu) | (((a >> 16) + (b >> 16)) << 16);
+    return vmin16(s, c);
 #endif
 }
 // bytes (sign(t1 bit 15), sign(t2 bit 15), sign(t1 bit 31), sign(t2 bit 31)) as 0x00 / 0xFF: PRMT in sign-replicating mode
@@ -118,7 +119,8 @@ VIT_HD void vit_metrics(uint32_t w, uint32_t E[8])
 // MC[p] = E[p] | E[p ^ DELTA] << 16.  Built directly in packed form: with A = s0 + s3, B = s1, C = s2 (one dot-product
 // instruction each) the pair (x, x) or (x, max - x) is one multiply-add, its complement (max, max) - pair one subtract, and
 // MC[p] = PA[p & 1] + PB[(p >> 1) & 1] + PC[p >> 2] (no carry between the halves: every sum is <= 1020).
-template <int DELTA> VIT_HD void vit_mc(uint32_t w, uint32_t (&MC)[8])
+// KM[p] = MC[p] + KOFF, the decision offsets of vit_acs (KOFF's halves <= 0x8000: every half of KM stays below 0x10000).
+template <int DELTA, uint32_t KOFF> VIT_HD void vit_mc(uint32_t w, uint32_t (&MC)[8], uint32_t (&KM)[8])
 {
 #if defined(__CUDA_ARCH__)
     const uint32_t A = __dp4a(w, 0x01000001u, 0u), B = __dp4a(w, 0x00000100u, 0u), C = __dp4a(w, 0x00010000u, 0u);
@@ -130,64 +132,76 @@ template <int DELTA> VIT_HD void vit_mc(uint32_t w, uint32_t (&MC)[8])
     const uint32_t PB0 = (DELTA & 2) ? B * 0xFFFF0001u + (255u << 16) : B * 0x00010001u;
     const uint32_t PC0 = (DELTA & 4) ? C * 0xFFFF0001u + (255u << 16) : C * 0x00010001u;
     const uint32_t PA[2] = {PA0, 0x01FE01FEu - PA0}, PB[2] = {PB0, 0x00FF00FFu - PB0}, PC[2] = {PC0, 0x00FF00FFu - PC0};
+    const uint32_t PK[2] = {PC[0] + KOFF, PC[1] + KOFF};
     uint32_t AB[4];
 #pragma unroll
     for (int q = 0; q < 4; q++) AB[q] = PA[q & 1] + PB[q >> 1];
 #pragma unroll
-    for (int p = 0; p < 8; p++) MC[p] = AB[p & 3] + PC[p >> 2];
+    for (int p = 0; p < 8; p++) { MC[p] = AB[p & 3] + PC[p >> 2]; KM[p] = AB[p & 3] + PK[p >> 2]; }
 }
+
+// The multiplicative inverse of 255 modulo 2^32.  A word of 0x00 / 0xFF bytes is 255 x the same word with 0x00 / 0x01 bytes, so
+// bytes * (VIT_INV255 << g) is that word shifted to bit g of every byte: one IMAD (FMA pipe) masks and places four decisions, and
+// summing such terms for distinct g is the OR of them.
+constexpr uint32_t VIT_INV255 = 0xFEFEFEFFu;
 
 // One ACS step from layout L_B to L_{(B+1)%6}.  Q: 32 packed metric registers; dlo/dhi: decision bits of new states
 // 0..31 / 32..63.
 template <int B> VIT_HD void vit_acs(uint32_t (&Q)[32], const uint32_t w, uint32_t& dlo, uint32_t& dhi)
 {
     uint32_t N[32];
+    // A packed minimum min(a + m, c) of candidate pairs is one VIADDMNMX: of the four candidate sums of a butterfly pair only the
+    // two that are a minimum's second operand are formed.
     // Decisions without predicates.  For a packed pair (a, b) of candidate metrics (every half in [0, 0x7FFF]) t = a + 0x7FFF7FFF - b has
     // bit 15 / 31 set exactly where b wins strictly ((a - b) > 0: ties keep the a = old[i] branch, viterbi.cpp:263-275) and no carry
-    // crosses the halves.  One PRMT in sign-replicating mode turns the two sign bits of two such words into four 0x00 / 0xFF bytes, one
-    // LOP3 masks them to bit g of every byte and ORs them into the step's decision word: 2 instructions per packed minimum like the
-    // predicated form (VIMNMX with two predicate outputs + two predicated adds), but nothing competes for the seven predicate registers
-    // (that form made the scheduler park predicates in general registers: ~45 extra instructions per step).
+    // crosses the halves.  With a = q + MC[p], that is t = q + KM[p] - b: one IADD3 from the old metric and the candidate b the
+    // minimum needs anyway, so a is never formed.  One PRMT in sign-replicating mode turns the two sign bits of two such words
+    // into four 0x00 / 0xFF bytes, and one IMAD with VIT_INV255 << g moves them to bit g of every byte and adds them into the step's
+    // decision word.  (A predicated form - VIMNMX with two predicate outputs + two predicated adds - made the scheduler park
+    // predicates in general registers: ~45 extra instructions per step.)
     // Decision layout of a step: group g (0..15) = the two packed minima that share their input registers, byte lane l (0..3) as listed
     // below; decision bit at word g >> 3, bit 8 l + (g & 7) (vit_dec_pos<B> is the inverse map for the traceback).
     uint32_t W[2] = {0u, 0u};
-#define VIT_T(a, b) ((a) + 0x7FFF7FFFu - (b))
-#define VIT_PUT(g, t1, t2) do { W[(g) >> 3] |= vit_signbytes(t1, t2) & (0x01010101u << ((g) & 7)); } while (0)
+#define VIT_PUT(g, t1, t2) do { W[(g) >> 3] += vit_signbytes(t1, t2) * (VIT_INV255 << ((g) & 7)); } while (0)
     if constexpr (B < 5) {
         constexpr int delta = vit_pat(1 << B);   // pattern change when butterfly bit B flips
-        uint32_t MC[8];
-        vit_mc<delta>(w, MC);
+        uint32_t MC[8], KM[8];
+        vit_mc<delta, 0x7FFF7FFFu>(w, MC, KM);
 #pragma unroll
         for (int j = 0; j < 16; j++) {
             const int ilo = vit_insert_zero(j, B);            // butterfly with bit B = 0; its SIMD partner is ilo + (1<<B)
             const int ra = vit_remove_bit(ilo, B), rb = vit_remove_bit(ilo + 32, B);
             const int p = vit_pat(ilo);
-            const uint32_t m0 = Q[ra] + MC[p], m1 = Q[rb] + MC[p ^ 7], m2 = Q[ra] + MC[p ^ 7], m3 = Q[rb] + MC[p];
+            // candidates m0 = Q[ra] + MC[p], m1 = Q[rb] + MC[p ^ 7], m2 = Q[ra] + MC[p ^ 7], m3 = Q[rb] + MC[p]
+            const uint32_t m1 = Q[rb] + MC[p ^ 7], m3 = Q[rb] + MC[p];
             const int ne = 2 * ilo;                           // new states: (ne, ne + (2 << B)) from (m0, m1), (ne + 1, ne + 1 + (2 << B)) from (m2, m3)
-            N[vit_remove_bit(ne, B + 1)] = vmin16(m0, m1);
-            N[vit_remove_bit(ne + 1, B + 1)] = vmin16(m2, m3);
-            VIT_PUT(j, VIT_T(m0, m1), VIT_T(m2, m3));         // lanes: ne, ne + 1, ne + (2 << B), ne + 1 + (2 << B)
+            N[vit_remove_bit(ne, B + 1)] = vaddmin16(Q[ra], MC[p], m1);
+            N[vit_remove_bit(ne + 1, B + 1)] = vaddmin16(Q[ra], MC[p ^ 7], m3);
+            VIT_PUT(j, Q[ra] + KM[p] - m1, Q[ra] + KM[p ^ 7] - m3);   // lanes: ne, ne + 1, ne + (2 << B), ne + 1 + (2 << B)
         }
     } else {
-        // L_5: register i = (old[i], old[i+32]); result register i = (new[2i], new[2i+1]) = layout L_0
-        uint32_t XC[8];
-        vit_mc<7>(w, XC);
+        // L_5: register i = (old[i], old[i+32]); result register i = (new[2i], new[2i+1]) = layout L_0.  With m = E[p] of butterfly i,
+        // a = Q[i] + (m, m) = (old[i] + m, old[i+32] + m) and b = swap(Q[i]) + (1020 - m, 1020 - m) = (old[i+32] + 1020 - m, old[i] + 1020 - m)
+        // hold the candidates of new[2i] in their low and of new[2i+1] in their high halves: N[i] = min(a, b).  In the high half the old[i]
+        // candidate is b's, so t = a - b + 0x80007FFF has bit 31 set where old[i+32] does NOT win strictly; XOR-ing the decision words
+        // with 0xFFFF0000 (byte lanes 2, 3) turns those bits into decisions.
+        uint32_t EE[8], KE[8];
+        vit_mc<0, 0x80007FFFu>(w, EE, KE);                     // EE[p] = (E[p], E[p]); EE[p ^ 7] = (1020 - E[p], 1020 - E[p])
 #pragma unroll
         for (int g = 0; g < 16; g++) {
             uint32_t t[2];
 #pragma unroll
             for (int h = 0; h < 2; h++) {
                 const int i = 2 * g + h, p = vit_pat(i);
-                const uint32_t x = dup_lo(Q[i]) + XC[p];        // (old[i] + m,        old[i] + 1020 - m)
-                const uint32_t y = dup_hi(Q[i]) + XC[p ^ 7];    // (old[i+32] + 1020-m, old[i+32] + m)
-                N[i] = vmin16(x, y);                            // (new[2i], new[2i+1])
-                t[h] = VIT_T(x, y);
+                const uint32_t b = swap16(Q[i]) + EE[p ^ 7];
+                N[i] = vaddmin16(Q[i], EE[p], b);              // (new[2i], new[2i+1])
+                t[h] = Q[i] + KE[p] - b;
             }
             VIT_PUT(g, t[0], t[1]);                             // lanes: 4g, 4g + 2, 4g + 1, 4g + 3
         }
+        W[0] ^= 0xFFFF0000u; W[1] ^= 0xFFFF0000u;
     }
 #undef VIT_PUT
-#undef VIT_T
     dlo = W[0]; dhi = W[1];
 #pragma unroll
     for (int r = 0; r < 32; r++) Q[r] = N[r];
