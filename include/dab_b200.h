@@ -86,7 +86,8 @@ typedef struct {
                                    enum is refused with DABB_E_ARG and the call changes nothing */
     int32_t sample_clock;       /* DABB_CLOCK_*: track each stream's sample-clock error and remove the phase ramp it puts on the softbits
                                    (see below); a value outside the enum is refused with DABB_E_ARG and the call changes nothing */
-    int32_t reserved[1];
+    int32_t acquisition;        /* DABB_ACQ_*: how a stream that is not synchronised finds the null symbol (see below); a value outside the enum
+                                   is refused with DABB_E_ARG and the call changes nothing */
 } dabb_options;
 
 /* Soft-decision demap of the OFDM demodulator, dabb_options.soft_demap; takes effect from the next step, and dabb_ofdm_demod uses the
@@ -136,6 +137,48 @@ typedef struct {
     int32_t frames;             /* n */
     int32_t reserved;
 } dabb_clock_result;
+
+/* Acquisition, dabb_options.acquisition; takes effect from the next step.  A stream in the middle of a search continues from its position
+ * under whichever method is set; dabb_stream_reset starts a new search.
+ * DABB_ACQ_REFERENCE (0, the default) is OFDMProcessor::run's notSynced state (ofdm-processor.cpp:253-323): a 50-sample mean of |Re|+|Im|
+ * below 0.5 sLevel.  During the null symbol that ratio is about sqrt(N / (S + N)), 0.71 at 0 dB SNR, so below about 2 dB the dip rarely
+ * crosses the threshold, and a narrowband interferer fills the null.
+ * DABB_ACQ_ROBUST (1) (replaces: none; it deviates from ofdm-processor.cpp:253-323 and phasereference.cpp:73-97) searches the spectrum:
+ *   span: from the stream's position p (logical), nb = min(floor((buf_len - (p - buf_start)) / 256), 784) consecutive blocks of 256
+ *     samples aligned to p; nb < 32 (or p outside the buffer): no search in this step, nothing changes.  Sample i of the span is
+ *     mixed with the oscillator as OFDMProcessor::getSamples mixes it, osc[(localPhase - (i + 1)(coarse + fine)) mod 2 048 000] (not at
+ *     all while both are 0);
+ *   block level: with w[n] = 0.5 - 0.5 c[n], c[n] = (float)cos(2 pi n / 256) from double, X = the 256-point DFT of w[n] y[n] (radix-2
+ *     decimation in time, every product and sum rounded) and P_k = Re^2 + Im^2 of bin k, |k| <= 87 (|f| <= 700 kHz), the level is
+ *     mean over k of log2(min(max(P_k, 2^-126), FLT_MAX)) (NaN reads as 2^-126): lane t of 32 sums k = t - 87, t - 55, ... in ascending
+ *     order, the 32 partials are added in lane order, then divided by 175.  log2 is a fixed series within 3e-7 of the exact value, and a level
+ *     depends neither on the batch size nor on the stream index;
+ *   decision: W_b = the sum of the levels of blocks b .. b + 8 in ascending order (nine blocks lie wholly inside the 2656-sample null at
+ *     any alignment); b* = the last b with the smallest W_b (in digital silence, where all are equal, its end); M = the ((nb - 1) / 2)-th smallest level; depth = (M - W_b* / 9) * 3.0103
+ *     dB.  A null is found when depth >= 1.2 dB (D) and b* + 11 <= nb;
+ *   found: the null ends at about p + 256 b* + 2480 (between 2304 and 2656 samples after the window's first sample when the window lies
+ *     in the null); the stream skips 256 b* + 2224 samples (tracking starts 256 samples before that estimate), localPhase advances by
+ *     the samples skipped times (coarse + fine) as getSamples would, and it is acquired: time synchronisation places the frame from
+ *     there as it does after the reference's search, with any placement.  When the step's buffer does not hold that frame the step
+ *     reports DABB_FRAME_NEED_SAMPLES with next_pos at the hand-off (the only case in which that status comes with a changed state);
+ *   not found: the stream skips 256 (nb - 11) samples, so that a null the buffer's end cut through is searched whole in the next step,
+ *     counts one acq_failed and reports DABB_FRAME_ACQUIRING;
+ *   either way sLevel becomes the span's mean |Re| + |Im| (block sums in lane order, then summed in double).
+ * Under DABB_ACQ_ROBUST the phase reference correlation (find_index) also excises narrowband interferers: between the forward transform
+ * of the window and the multiply by conj(PRS), with G the geometric mean of the 1536 in-band bin powers (same log2 and clamp; thread t of
+ * 128 sums its bins t + 128 c in ascending c, the 128 partials in thread order), every in-band bin with log2 P > log2 G + log2 20 (T = 20)
+ * and its two neighbours on each side (circularly) are set to 0.  A window with no such bin gives bit for bit the CIR and index of the
+ * reference correlation.  Against the float64 restatement (tests/acqref.py) a level is within 2e-5 (2e-5 times the amplitude ratio of a tone to
+ * the ensemble beside a tone: the float32 transform's error in the weak bins), a depth within 3.1 times that in dB. */
+enum { DABB_ACQ_REFERENCE = 0, DABB_ACQ_ROBUST = 1 };
+/* one stream in one step: tap 13 (all zero when the step ran with DABB_ACQ_REFERENCE) */
+typedef struct {
+    int32_t searched;           /* 1: the stream searched in this step */
+    int32_t blocks;             /* nb, the blocks analysed */
+    float depth_db;             /* depth of the best window */
+    int32_t excised;            /* bins zeroed in this step's phase reference window */
+    int64_t null_end;           /* logical position of the found null's estimated end (p + 256 b* + 2480), -1 when none was found */
+} dabb_acq_result;
 
 /* Diversity reception (replaces: none; the reference is one receiver with one input).  Coherent multi-channel receivers record one file
  * per antenna on a shared sample clock; decoded as neighbouring streams of one context, the antennas of one capture can be combined.
@@ -346,7 +389,8 @@ int dabb_profile_read(dabb_ctx* ctx, char* json_out, size_t cap);
  *  11 = dabb_clock_result [n_streams] of the last step (all zero when that step ran with sample_clock OFF); DABB_E_STATE until
  *       dabb_options.sample_clock has been set to DABB_CLOCK_TRACK once
  *  12 = dabb_combine_result [n_streams] of the last step (all zero when that step ran without a group); DABB_E_STATE until
- *       dabb_set_combining has formed a group of two or more streams once */
+ *       dabb_set_combining has formed a group of two or more streams once
+ *  13 = dabb_acq_result [n_streams] of the last step; DABB_E_STATE until dabb_options.acquisition has been set to DABB_ACQ_ROBUST once */
 int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes);
 
 /* ---------------------------------------------------------------------------------------------------------

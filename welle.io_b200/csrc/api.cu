@@ -169,6 +169,11 @@ struct dabb_ctx {
     DevBuf<CombGroup> d_comb_groups, d_comb_groups_full; DevBuf<CombItem> d_comb_items; DevBuf<int32_t> d_comb_gid, d_comb_row, d_comb_row_full;
     DevBuf<uint32_t> d_comb_lmask; DevBuf<float2> d_comb_r1; DevBuf<dabb_combine_result> d_comb_res; CombParams comb_op{};
     DevBuf<CombGroup> d_comb_groups_next; DevBuf<int32_t> d_comb_row_next; int comb_next_groups = 0, comb_next_grouped = 0; bool comb_staged = false;
+    // robust acquisition (acquisition = DABB_ACQ_ROBUST, acq.cu), allocated when the option is first set: the cosine table of the block
+    // transform, each stream's search span, the block levels and envelope sums [S][NB_MAX], the bins the excising find_index instance
+    // zeroed [S], and the step's records (tap 13, with `excised` taken from d_acq_exc when it is read)
+    int acquisition = DABB_ACQ_REFERENCE; DevBuf<float> d_acq_cos, d_acq_level, d_acq_l1; DevBuf<AcqJob> d_acq_job; DevBuf<int32_t> d_acq_exc;
+    DevBuf<dabb_acq_result> d_acq_res;
 };
 
 namespace {
@@ -293,6 +298,63 @@ __global__ void acquire_kernel(StreamState* st, const float2* iq, int64_t stride
         break;
     }
     checkpoint();      // acquired: tracking starts here; not acquired: the next call continues the search from here
+}
+
+// Robust acquisition (DABB_ACQ_ROBUST, acq_core.cuh), in place of acquire_kernel: the span each searching stream analyses in this step,
+// from its position to the end of its buffer, at most NB_MAX blocks; fewer than MIN_BLOCKS: no search
+__global__ void acq_plan_kernel(const StreamState* st, const int64_t* buf_start, int64_t buf_len, int S, AcqJob* job)
+{
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= S) return;
+    const StreamState z = st[s];
+    AcqJob j{};
+    j.rel = z.pos - buf_start[s];
+    if (!z.acquired && j.rel >= 0 && j.rel < buf_len) {
+        const int64_t nb = (buf_len - j.rel) / dabb_acq::BLK;
+        j.nb = nb < dabb_acq::MIN_BLOCKS ? 0 : (int32_t)(nb < dabb_acq::NB_MAX ? nb : dabb_acq::NB_MAX);
+    }
+    j.lp = z.local_phase; j.phase = z.coarse + z.fine;
+    job[s] = j;
+}
+
+// the decision of one searching stream (one CTA): the first window of WIN blocks with the smallest level sum, its depth below the span's
+// median level, and the hand-off to time synchronisation.  Every stream's tap-13 record of the step is written here.
+__global__ void __launch_bounds__(256)
+acq_decide_kernel(StreamState* st, const AcqJob* job, const int64_t* buf_start, const float* level, const float* l1sum, dabb_acq_result* res)
+{
+    using namespace dabb_acq;
+    __shared__ float lv[NB_MAX];
+    __shared__ float med;
+    const int s = blockIdx.x, t = threadIdx.x;
+    const AcqJob j = job[s];
+    if (!j.nb) { if (t == 0) res[s] = dabb_acq_result{0, 0, 0.f, 0, -1}; return; }
+    const int nb = j.nb;
+    for (int i = t; i < nb; i += blockDim.x) lv[i] = level[(int64_t)s * NB_MAX + i];
+    __syncthreads();
+    // median: the level with exactly k = (nb - 1) / 2 levels below it (levels are finite, so the value is well defined)
+    const int k = (nb - 1) / 2;
+    for (int i = t; i < nb; i += blockDim.x) {
+        int less = 0, leq = 0;
+        for (int m = 0; m < nb; m++) { less += lv[m] < lv[i]; leq += lv[m] <= lv[i]; }
+        if (less <= k && k < leq) med = lv[i];
+    }
+    __syncthreads();
+    if (t) return;
+    int best = 0; float wmin = window_sum(lv, 0);
+    for (int b = 1; b + WIN <= nb; b++) { const float w = window_sum(lv, b); if (w <= wmin) { wmin = w; best = b; } }     // last of equal minima
+    const float depth = depth_db(med, wmin);
+    const bool found = is_found(depth, best, nb);
+    double env = 0.0;
+    for (int b = 0; b < nb; b++) env += (double)l1sum[(int64_t)s * NB_MAX + b];
+    StreamState z = st[s];
+    const int64_t skip = found ? (int64_t)best * BLK + NULL_END - LEAD : (int64_t)(nb - KEEP) * BLK;
+    z.pos += skip;
+    z.local_phase = mod_rate((int64_t)z.local_phase - skip * j.phase);
+    z.started = 1;
+    z.slevel = (float)(env / ((double)nb * BLK));
+    if (found) z.acquired = 1; else z.acq_failed++;
+    st[s] = z;
+    res[s] = dabb_acq_result{1, nb, depth, 0, found ? buf_start[s] + j.rel + (int64_t)best * BLK + NULL_END : -1};
 }
 
 __global__ void plan_kernel(StreamState* st, StepScratch* scr, const int64_t* buf_start, int64_t buf_len, int S,
@@ -1144,15 +1206,30 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     prof_mark(ctx, "__step_begin");
     const int tb = 128, gb = (S + tb - 1) / tb;
     // ---------------- lane A
-    acquire_kernel<<<(S + 31) / 32, 32, 0, A>>>(ctx->d_state, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, S);
-    if ((rc = check_launch(ctx, "acquire_kernel"))) return rc;
+    const bool robust = ctx->acquisition == DABB_ACQ_ROBUST;
+    if (robust) {       // the spectral null search of every stream that is not tracking, then the same hand-off to time sync
+        CK(cudaMemsetAsync(ctx->d_acq_exc, 0, sizeof(int32_t) * S, A));
+        acq_plan_kernel<<<gb, tb, 0, A>>>(ctx->d_state, ctx->d_buf_start, io->buf_len, S, ctx->d_acq_job);
+        if ((rc = check_launch(ctx, "acq_plan_kernel"))) return rc;
+        launch_acq_levels(ctx->d_acq_job, iq, stride, ctx->dev.osc, ctx->d_acq_cos, S, ctx->d_acq_level, ctx->d_acq_l1, A);
+        if ((rc = check_launch(ctx, "acq_level_kernel"))) return rc;
+        acq_decide_kernel<<<S, 256, 0, A>>>(ctx->d_state, ctx->d_acq_job, ctx->d_buf_start, ctx->d_acq_level, ctx->d_acq_l1, ctx->d_acq_res);
+        if ((rc = check_launch(ctx, "acq_decide_kernel"))) return rc;
+    } else {
+        if (ctx->d_acq_res) {     // tap 13: nothing searched robustly in this step
+            CK(cudaMemsetAsync(ctx->d_acq_res, 0, sizeof(dabb_acq_result) * S, A));
+            CK(cudaMemsetAsync(ctx->d_acq_exc, 0, sizeof(int32_t) * S, A));
+        }
+        acquire_kernel<<<(S + 31) / 32, 32, 0, A>>>(ctx->d_state, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, S);
+        if ((rc = check_launch(ctx, "acquire_kernel"))) return rc;
+    }
     plan_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, ctx->d_buf_start, io->buf_len, S, d_win, d_nco_sync, d_active);
     if ((rc = check_launch(ctx, "plan_kernel"))) return rc;
     SyncParams sp{}; sp.iq = iq; sp.stride = stride; sp.win_start = d_win; sp.nco = d_nco_sync; sp.active = d_active; sp.index_out = d_index; sp.cir_out = ctx->d_cir; sp.n = S;
     sp.fic_ratio = ctx->d_fic_ratio; sp.coarse_out = ctx->disable_coarse ? nullptr : ctx->d_coarse.get(); sp.placement = ctx->placement; sp.freqsync = ctx->freqsync;
     sp.cir_work = ctx->d_cir_work;
-    launch_find_index(ctx->dev, sp, A, 0);
-    if ((rc = check_launch(ctx, "find_index_kernel"))) return rc;
+    launch_find_index(ctx->dev, sp, A, 0, robust ? ctx->d_acq_exc.get() : nullptr);
+    if ((rc = check_launch(ctx, robust ? "find_index_excise_kernel" : "find_index_kernel"))) return rc;
     launch_find_index(ctx->dev, sp, A, 1);
     if ((rc = check_launch(ctx, "find_search_kernel"))) return rc;
     if (sp.coarse_out) {
@@ -1421,6 +1498,14 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
         if (!ctx->d_clock_res) { ctx->err = "tap 11 needs dabb_options.sample_clock to have been set"; return DABB_E_STATE; }
         const size_t n = sizeof(dabb_clock_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_clock_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
     }
+    if (what == 13) {
+        if (!ctx->d_acq_res) { ctx->err = "tap 13 needs dabb_options.acquisition to have been set to DABB_ACQ_ROBUST"; return DABB_E_STATE; }
+        std::vector<dabb_acq_result> r(ctx->S); std::vector<int32_t> exc(ctx->S);
+        CK(cudaMemcpy(r.data(), ctx->d_acq_res, sizeof(dabb_acq_result) * ctx->S, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(exc.data(), ctx->d_acq_exc, sizeof(int32_t) * ctx->S, cudaMemcpyDeviceToHost));
+        for (int s = 0; s < ctx->S; s++) r[s].excised = exc[s];
+        const size_t n = sizeof(dabb_acq_result) * ctx->S; memcpy(host_out, r.data(), bytes < n ? bytes : n); return 0;
+    }
     if (what == 12) {
         if (!ctx->d_comb_res) { ctx->err = "tap 12 needs dabb_set_combining to have formed a group"; return DABB_E_STATE; }
         const size_t n = sizeof(dabb_combine_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_comb_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
@@ -1520,7 +1605,8 @@ int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
 {
     if (!ctx || !opt || opt->fft_placement < 0 || opt->fft_placement > 2 || opt->freqsync_method < 0 || opt->freqsync_method > 2
         || (opt->soft_demap != DABB_DEMAP_REFERENCE && opt->soft_demap != DABB_DEMAP_WEIGHTED)
-        || (opt->sample_clock != DABB_CLOCK_OFF && opt->sample_clock != DABB_CLOCK_TRACK)) return DABB_E_ARG;
+        || (opt->sample_clock != DABB_CLOCK_OFF && opt->sample_clock != DABB_CLOCK_TRACK)
+        || (opt->acquisition != DABB_ACQ_REFERENCE && opt->acquisition != DABB_ACQ_ROBUST)) return DABB_E_ARG;
     if (opt->decode_tii && !ctx->d_tii_res) {       // first use of TII: its buffers (64 KB per stream), zeroed = no open combinations
         cudaSetDevice(ctx->device);
         sync_all(ctx);
@@ -1555,8 +1641,25 @@ int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
         if ((rc = dalloc(ctx, ctx->d_clock_res, (size_t)ctx->S))) { ctx->d_clock_frame.reset(); return rc; }      // last: it marks tracking as available
         CK(cudaStreamSynchronize(ctx->stream));
     }
+    if (opt->acquisition == DABB_ACQ_ROBUST && !ctx->d_acq_res) {     // first use of the robust search: its tables, scratch and records
+        cudaSetDevice(ctx->device);
+        sync_all(ctx);
+        const size_t S = (size_t)ctx->S;
+        float cos_tab[dabb_acq::BLK];
+        dabb_acq::make_cos_table(cos_tab);
+        int rc;
+        if ((rc = dalloc(ctx, ctx->d_acq_cos, dabb_acq::BLK)) || (rc = dalloc(ctx, ctx->d_acq_job, S)) || (rc = dalloc(ctx, ctx->d_acq_level, S * dabb_acq::NB_MAX)) ||
+            (rc = dalloc(ctx, ctx->d_acq_l1, S * dabb_acq::NB_MAX)) || (rc = dalloc(ctx, ctx->d_acq_exc, S))) {
+            ctx->d_acq_cos.reset(); ctx->d_acq_job.reset(); ctx->d_acq_level.reset(); ctx->d_acq_l1.reset(); ctx->d_acq_exc.reset();
+            return rc;
+        }
+        CK(cudaMemcpyAsync(ctx->d_acq_cos, cos_tab, sizeof cos_tab, cudaMemcpyHostToDevice, ctx->stream));
+        if ((rc = dalloc(ctx, ctx->d_acq_res, S))) return rc;      // last: it marks the search as available
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
     ctx->disable_coarse = opt->disable_coarse != 0; ctx->placement = opt->fft_placement; ctx->freqsync = opt->freqsync_method; ctx->decode_tii = opt->decode_tii != 0;
     ctx->count_ber = opt->count_bit_errors != 0; ctx->soft_demap = opt->soft_demap; ctx->sample_clock = opt->sample_clock;
+    ctx->acquisition = opt->acquisition;
     return DABB_OK;
 }
 

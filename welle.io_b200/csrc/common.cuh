@@ -10,6 +10,7 @@
 #include "ofdm_mask.cuh"
 #include "clock_core.cuh"
 #include "combine_core.cuh"
+#include "acq_core.cuh"
 
 namespace dabb {
 
@@ -87,7 +88,7 @@ struct SyncParams {
 void launch_ofdm_demod(const DevTables& tb, const OfdmParams& p, int fft_mode, cudaStream_t st);
 int ofdm_tail_frames(int n_frames);
 constexpr int OFDM_TAIL_GROUPS = 5;              // CTAs per tail frame (15 data symbols each): the best of 5 / 15 / 25 before the port to H100
-void launch_find_index(const DevTables& tb, const SyncParams& p, cudaStream_t st, int part = -1);
+void launch_find_index(const DevTables& tb, const SyncParams& p, cudaStream_t st, int part = -1, int32_t* excised = nullptr);
 void launch_tii_spectra(const DevTables& tb, const float2* iq, int64_t stride, const int64_t* prs_start, const int32_t* nco_frame, const int32_t* active,
                         const float2* nulls, float2* out, int n, cudaStream_t st);
 void launch_coarse(const DevTables& tb, const float2* iq, int64_t stride, const int64_t* prs_start, int n, int freqsync, int32_t* out, cudaStream_t st);
@@ -159,6 +160,17 @@ struct SurveyParams {
 cudaError_t launch_survey(const SurveyParams& p, int log2n, int64_t n_chunks, int n_inputs, cudaStream_t st);
 // psd[i][j] = scale * sum over the chunks of input i of part at bin j (double, ascending chunk order)
 void launch_survey_sum(const float* part, int64_t n_chunks, int log2n, int n_inputs, double scale, float* psd, cudaStream_t st);
+
+// ---- robust acquisition (acq.cu, acq_core.cuh): the span one searching stream analyses in a step (acq_plan_kernel in api.cu) ----
+struct AcqJob {
+    int64_t rel;            // the search start (the stream's position) relative to its buffer
+    int32_t nb;             // blocks of 256 samples analysed (0: the stream does not search in this step)
+    int32_t lp, phase;      // NCO: sample i of the span is mixed with osc[(lp - (i + 1) phase) mod 2 048 000]; none when both are 0
+    int32_t pad;
+};
+// levels [S][NB_MAX] and envelope sums [S][NB_MAX] of every analysed block; cos_tab: dabb_acq::make_cos_table
+void launch_acq_levels(const AcqJob* job, const float2* iq, int64_t stride, const float2* osc, const float* cos_tab, int S,
+                       float* level, float* l1sum, cudaStream_t st);
 
 // ---- host-side table builders (tables.cpp) ----
 struct HostTables {

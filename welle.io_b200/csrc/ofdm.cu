@@ -776,9 +776,51 @@ coarse_kernel(DevTables tb, const float2* iq, int64_t stride, const int64_t* prs
     coarse_estimate(tb, sm, iq + (int64_t)f * stride, prs_start[f], nco, xi, t, freqsync, out + f);
 }
 
-template <bool NCO>
-__global__ void __launch_bounds__(OFDM_THREADS, 5)
-find_index_kernel(DevTables tb, SyncParams p)
+// interferer excision (DABB_ACQ_ROBUST, acq_core.cuh) on the window's spectrum, bins t + 128 c in v[c]: G is the geometric mean of the
+// in-band bin powers (per thread in ascending c, the 128 partials in thread order); every in-band bin with power above T G and its
+// EXC_NEIGH neighbours on each side (circular) are zeroed.  A window with no such bin is left untouched, bit for bit.  Thread 0 writes
+// the number of zeroed bins.
+__device__ __forceinline__ void excise_bins(float2 (&v)[16], int t, int32_t* excised)
+{
+    using namespace dabb_acq;
+    __shared__ float part[EXC_THREADS];
+    __shared__ uint32_t mark[TU / 32];
+    __shared__ int total;
+    float pw[16];
+    float s = 0.f;
+#pragma unroll
+    for (int c = 0; c < 16; c++) {
+        pw[c] = __fadd_rn(__fmul_rn(v[c].x, v[c].x), __fmul_rn(v[c].y, v[c].y));
+        if (in_band(t + 128 * c)) s = __fadd_rn(s, log2_pos(clamp_power(pw[c])));        // exc_partial
+    }
+    part[t] = s;
+    if (t < TU / 32) mark[t] = 0u;
+    if (t == 0) total = 0;
+    __syncthreads();
+    const float limit = exc_limit(part);
+    bool any = false;
+#pragma unroll
+    for (int c = 0; c < 16; c++) {
+        const int bin = t + 128 * c;
+        if (exc_over(pw[c], bin, limit)) {
+            any = true;
+            for (int d = -EXC_NEIGH; d <= EXC_NEIGH; d++) { const int b = (bin + d) & (TU - 1); atomicOr(&mark[b >> 5], 1u << (b & 31)); }
+        }
+    }
+    if (!__syncthreads_or(any)) { if (t == 0) *excised = 0; return; }      // CTA-uniform: nothing to excise
+    int n = 0;
+#pragma unroll
+    for (int c = 0; c < 16; c++) {
+        const int bin = t + 128 * c;
+        if ((mark[bin >> 5] >> (bin & 31)) & 1u) { v[c] = make_float2(0.f, 0.f); n++; }
+    }
+    atomicAdd(&total, n);
+    __syncthreads();
+    if (t == 0) *excised = total;
+}
+
+template <bool NCO, bool EXCISE>
+__device__ __forceinline__ void find_index_body(const DevTables& tb, const SyncParams& p, int32_t* excised)
 {
     extern __shared__ __align__(16) unsigned char smraw[];
     SyncSmem& sm = *reinterpret_cast<SyncSmem*>(smraw);
@@ -791,6 +833,7 @@ find_index_kernel(DevTables tb, SyncParams p)
     const XIdx xi = make_xidx(t);
     float2 v[16];
     fft2048_from_global(src, 0, v, sm.o, t, xi, tb, nco, tb.tw_fwd + TwLayout::C5);
+    if constexpr (EXCISE) excise_bins(v, t, excised + f);
     // res = X * conj(ref), written in natural order into the exchange buffer (free between the two transforms)
     float2* scratch = sm.o.xbuf;
     __syncthreads();             // pass C of the forward transform has read xbuf
@@ -846,6 +889,21 @@ find_index_kernel(DevTables tb, SyncParams p)
         const double m = __dsqrt_rn(__dadd_rn(__dmul_rn((double)re, (double)re), __dmul_rn((double)im, (double)im)));
         cw[t + 128 * c] = (float)m;
     }
+}
+
+template <bool NCO>
+__global__ void __launch_bounds__(OFDM_THREADS, 5)
+find_index_kernel(DevTables tb, SyncParams p)
+{
+    find_index_body<NCO, false>(tb, p, nullptr);
+}
+
+// the same with the interferer excision of DABB_ACQ_ROBUST; excised[f]: the bins zeroed in window f
+template <bool NCO>
+__global__ void __launch_bounds__(OFDM_THREADS, 5)
+find_index_excise_kernel(DevTables tb, SyncParams p, int32_t* excised)
+{
+    find_index_body<NCO, true>(tb, p, excised);
 }
 
 // findIndex, second part: the placement search over the 2048 magnitudes of one window (phasereference.cpp:93-211) for the
@@ -1114,11 +1172,16 @@ void launch_coarse(const DevTables& tb, const float2* iq, int64_t stride, const 
 
 // part: 0 transforms -> magnitudes, 1 placement search -> index, 2 coarse estimate where the FIC counter asks for it, -1 all three
 // Time sync always uses the exact arithmetic, whatever the context's fft_mode: its integer result feeds the closed loop.
-void launch_find_index(const DevTables& tb, const SyncParams& p, cudaStream_t st, int part)
+// excised (or nullptr): the transforms excise interferers (DABB_ACQ_ROBUST) and record the zeroed bins per window
+void launch_find_index(const DevTables& tb, const SyncParams& p, cudaStream_t st, int part, int32_t* excised)
 {
     const dim3 grid(p.n), block(OFDM_THREADS);
     const bool nco = p.nco != nullptr;
-    if (part < 0 || part == 0) {
+    if ((part < 0 || part == 0) && excised) {
+        const size_t sm = sizeof(OfdmSmem);
+        if (nco) { set_smem(find_index_excise_kernel<true>, sm); find_index_excise_kernel<true><<<grid, block, sm, st>>>(tb, p, excised); }
+        else { set_smem(find_index_excise_kernel<false>, sm); find_index_excise_kernel<false><<<grid, block, sm, st>>>(tb, p, excised); }
+    } else if (part < 0 || part == 0) {
         const size_t sm = sizeof(OfdmSmem);
         if (nco) { set_smem(find_index_kernel<true>, sm); find_index_kernel<true><<<grid, block, sm, st>>>(tb, p); }
         else { set_smem(find_index_kernel<false>, sm); find_index_kernel<false><<<grid, block, sm, st>>>(tb, p); }

@@ -20,6 +20,7 @@ FFT_EXACT, FFT_FMA = 0, 1
 NCO_EXACT, NCO_FAST = 0, 1
 DEMAP_REFERENCE, DEMAP_WEIGHTED = 0, 1
 CLOCK_OFF, CLOCK_TRACK = 0, 1
+ACQ_REFERENCE, ACQ_ROBUST = 0, 1
 IQ_CF32, IQ_U8, IQ_S8, IQ_S16LE, IQ_S16BE = 0, 1, 2, 3, 4
 FRAME_DECODED, FRAME_NEED_SAMPLES, FRAME_NO_SYNC, FRAME_ACQUIRING = 0, 1, 2, 3
 
@@ -41,6 +42,8 @@ class Options(C.Structure):
     soft_demap = property(lambda self: self.reserved[0], lambda self, v: self.reserved.__setitem__(0, v))
     # dabb_options.sample_clock, the former reserved[1]
     sample_clock = property(lambda self: self.reserved[1], lambda self, v: self.reserved.__setitem__(1, v))
+    # dabb_options.acquisition, the former reserved[2]
+    acquisition = property(lambda self: self.reserved[2], lambda self, v: self.reserved.__setitem__(2, v))
 
 
 PLACEMENT_THRESHOLD_BEFORE_PEAK, PLACEMENT_STRONGEST_PEAK, PLACEMENT_EARLIEST_PEAK_WITH_BINNING = 0, 1, 2
@@ -85,6 +88,9 @@ assert CLOCK_DTYPE.itemsize == 16
 MAX_BRANCHES = 8
 COMBINE_DTYPE = np.dtype([("members", "<i4"), ("mask", "<u4"), ("noise", "<f4"), ("reserved", "<i4")])
 assert COMBINE_DTYPE.itemsize == 16
+# dabb_acq_result: one stream's robust null search and phase reference excision of one step (tap 13)
+ACQ_DTYPE = np.dtype([("searched", "<i4"), ("blocks", "<i4"), ("depth_db", "<f4"), ("excised", "<i4"), ("null_end", "<i8")])
+assert ACQ_DTYPE.itemsize == 24
 
 
 class IO(C.Structure):
@@ -374,12 +380,15 @@ class Context:
         return v.value
 
     def set_options(self, disable_coarse=True, fft_placement=0, freqsync_method=0, decode_tii=False, count_bit_errors=False, soft_demap=DEMAP_REFERENCE,
-                    sample_clock=CLOCK_OFF):
+                    sample_clock=CLOCK_OFF, acquisition=ACQ_REFERENCE):
         """soft_demap: DEMAP_REFERENCE (the reference's demap) or DEMAP_WEIGHTED (weak carriers scaled by their level over the symbol's
         geometric-mean level, see dabb_options.soft_demap); sample_clock: CLOCK_OFF or CLOCK_TRACK (each stream's sample-clock error
-        estimated from its frame timing and its phase ramp removed from the softbits, see dabb_options.sample_clock)"""
+        estimated from its frame timing and its phase ramp removed from the softbits, see dabb_options.sample_clock); acquisition:
+        ACQ_REFERENCE (the reference's envelope-dip null search) or ACQ_ROBUST (the null found from the spectral level of 256-sample
+        blocks, and narrowband interferers excised from the phase reference correlation, see dabb_options.acquisition)"""
         o = Options(); o.disable_coarse, o.fft_placement, o.freqsync_method, o.decode_tii = int(disable_coarse), int(fft_placement), int(freqsync_method), int(decode_tii)
         o.count_bit_errors, o.soft_demap, o.sample_clock = int(count_bit_errors), int(soft_demap), int(sample_clock)
+        o.acquisition = int(acquisition)
         self._ck(self.lib.dabb_set_options(self.h, C.byref(o)))
 
     def read_tap(self, what, stride=0):
@@ -387,7 +396,7 @@ class Context:
         4 TII spectra (PRS, null symbol), 5 frame results, 6 FIBs, 7 logical frames [S, MAX_SUBCH, 4, stride] and 8 superframes
         [S, MAX_SUBCH, stride] of the last step (also after process_async), 9 TII measurements (TII_DTYPE per stream), 10 channel bit
         errors (BER_DTYPE per stream), 11 sample-clock estimates (CLOCK_DTYPE per stream), 12 diversity combinations (COMBINE_DTYPE per
-        stream)"""
+        stream), 13 robust acquisition (ACQ_DTYPE per stream)"""
         if what == 7:
             out = np.zeros((self.n_streams, MAX_SUBCH, 4, stride), np.uint8)
         elif what == 8:
@@ -412,6 +421,8 @@ class Context:
             out = np.zeros(self.n_streams, CLOCK_DTYPE)
         elif what == 12:
             out = np.zeros(self.n_streams, COMBINE_DTYPE)
+        elif what == 13:
+            out = np.zeros(self.n_streams, ACQ_DTYPE)
         else:
             out = np.zeros((self.n_streams, TU), np.float32)
         self._ck(self.lib.dabb_read_tap(self.h, what, _vp(out), C.c_size_t(out.nbytes)))

@@ -3,7 +3,7 @@
  * wideband file, --rate), on one GPU.
  *
  *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock]
- *                [--diversity N] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file1 [file2 ...]
+ *                [--acq robust|reference] [--diversity N] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file1 [file2 ...]
  *
  * What `welle-cli -f FILE -D` does for one recording (welle-cli.cpp:215-235,612-707: dump the FIC, tune to the first audio
  * service, dump its logical frames) done for all files in lock-step: every iteration hands each stream's next window of samples
@@ -28,6 +28,12 @@
  * --offset auto survey and confirmation contexts included: each stream estimates its recording's sample-clock error from its frame
  * timing and the demodulator removes the phase ramp it puts on the softbits.  Every decoded frame adds one line "ppm applied_ppm frames"
  * (tap 11) to DIR/<name>.clk.
+ *
+ * --acq robust|reference: how a stream that is not synchronised finds the null symbol (dabb_options.acquisition) in every context the
+ * driver creates, the --scan / --offset auto survey and confirmation contexts included.  reference (the default) is the reference's
+ * envelope-dip search and leaves the options untouched; robust finds the null from the spectral level of 256-sample blocks, down to
+ * about 0 dB SNR and beside strong narrowband interferers, and excises such interferers from the phase reference correlation
+ * (DABB_ACQ_ROBUST).  Every step in which a stream searched adds one line "blocks depth_db found" (tap 13) to DIR/<name>.acq.
  *
  * --diversity N: consecutive runs of N files are the antennas of one capture (one coherent receiver's files: same rate, same first
  * sample); the first file of each run leads its group (dabb_set_combining) and decodes from the noise-weighted sum of the group's
@@ -82,6 +88,7 @@ namespace {
 struct Stream {
     std::string path, name; FILE* in = nullptr; FILE* fic = nullptr; FILE* msc = nullptr; FILE* rs = nullptr; FILE* tii = nullptr; FILE* ber = nullptr; FILE* clk = nullptr;
     FILE* div = nullptr;                                          /* --diversity: a group leader's combinations */
+    FILE* acq = nullptr;                                          /* --acq robust: the null searches */
     int64_t buf_start = 0, have = 0, pos = 0, acq_need = 0;      /* logical sample indices; `have` samples are buffered from buf_start */
     bool tracking = false, eof = false, done = false;
     std::unique_ptr<dabb_host::FigDb> db{new dabb_host::FigDb()};
@@ -104,6 +111,7 @@ struct Outputs {
     std::vector<dabb_frame_result> res; std::vector<uint8_t> fibs, msc, sf; std::vector<dabb_tii_result> tres; std::vector<dabb_ber_result> bres;
     std::vector<dabb_clock_result> cres;        /* tap 11, read after every step when not empty (--clock) */
     std::vector<dabb_combine_result> dres;      /* tap 12, read after every step when not empty (--diversity) */
+    std::vector<dabb_acq_result> ares;          /* tap 13, read after every step when not empty (--acq robust) */
 };
 
 /* the receiver position after one step's result r of stream s: 0 = the stream ended, 1 = no frame decoded, 2 = a frame was decoded */
@@ -126,6 +134,10 @@ int advance(dabb_ctx* ctx, Stream& z, int s, const dabb_frame_result& r, int64_t
 bool handle_result(dabb_ctx* ctx, Stream& z, int s, const Outputs& o, bool tii, bool ber, int64_t TF)
 {
     const dabb_frame_result& r = o.res[(size_t)s];
+    if (z.acq && o.ares[(size_t)s].searched) {
+        const dabb_acq_result& q = o.ares[(size_t)s];
+        fprintf(z.acq, "%d %.3f %d\n", q.blocks, q.depth_db, q.null_end >= 0 ? 1 : 0);
+    }
     if (tii)
         for (int i = 0; i < o.tres[(size_t)s].count; i++) {
             const auto& m = o.tres[(size_t)s].m[i];
@@ -218,6 +230,7 @@ bool step(dabb_ctx* ctx, Outputs& o, std::vector<int64_t>& buf_start, const floa
     if (ber && dabb_read_tap(ctx, 10, o.bres.data(), o.bres.size() * sizeof(dabb_ber_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     if (!o.cres.empty() && dabb_read_tap(ctx, 11, o.cres.data(), o.cres.size() * sizeof(dabb_clock_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     if (!o.dres.empty() && dabb_read_tap(ctx, 12, o.dres.data(), o.dres.size() * sizeof(dabb_combine_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
+    if (!o.ares.empty() && dabb_read_tap(ctx, 13, o.ares.data(), o.ares.size() * sizeof(dabb_acq_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     return true;
 }
 
@@ -334,15 +347,15 @@ bool run_wide(dabb_ctx* ctx, std::vector<Stream>& st, std::vector<Wide>& wf, int
 
 std::string base_name(const std::string& path) { const size_t slash = path.find_last_of('/'); return slash == std::string::npos ? path : path.substr(slash + 1); }
 
-/* a context of the scan with dabb_options.soft_demap = soft (--soft) and sample_clock = clock (--clock); the other options as cfg gives
- * them; false on an error */
-static bool create_scan_ctx(const dabb_config& cfg, int soft, int clock, dabb_ctx** ctx)
+/* a context of the scan with dabb_options.soft_demap = soft (--soft), sample_clock = clock (--clock) and acquisition = acq (--acq); the
+ * other options as cfg gives them; false on an error */
+static bool create_scan_ctx(const dabb_config& cfg, int soft, int clock, int acq, dabb_ctx** ctx)
 {
     if (dabb_create(&cfg, ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return false; }
-    if (soft == DABB_DEMAP_REFERENCE && clock == DABB_CLOCK_OFF) return true;
+    if (soft == DABB_DEMAP_REFERENCE && clock == DABB_CLOCK_OFF && acq == DABB_ACQ_REFERENCE) return true;
     dabb_options op; memset(&op, 0, sizeof op);
     op.disable_coarse = cfg.disable_coarse; op.fft_placement = cfg.fft_placement; op.freqsync_method = cfg.freqsync_method; op.soft_demap = soft;
-    op.sample_clock = clock;
+    op.sample_clock = clock; op.acquisition = acq;
     if (dabb_set_options(*ctx, &op) == DABB_OK) return true;
     fprintf(stderr, "batch_decode: %s\n", dabb_last_error(*ctx));
     dabb_destroy(*ctx);
@@ -351,7 +364,7 @@ static bool create_scan_ctx(const dabb_config& cfg, int soft, int clock, dabb_ct
 }
 
 /* --scan: the ensembles of every file (ascending offset, per file), as the streams of their confirmation decode; false on an error */
-bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int device, int soft, int clock, std::vector<std::vector<Stream>>& found)
+bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int device, int soft, int clock, int acq, std::vector<std::vector<Stream>>& found)
 {
     const int64_t TF = DABB_TF;
     const int bps = bytes_per_sample(fmt);
@@ -383,7 +396,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
     dabb_config cfg; memset(&cfg, 0, sizeof cfg);
     cfg.abi_version = DABB_ABI_VERSION; cfg.device = device; cfg.n_streams = 1; cfg.transmission_mode = 1;
     dabb_ctx* ctx = nullptr;
-    if (!create_scan_ctx(cfg, soft, clock, &ctx)) return false;
+    if (!create_scan_ctx(cfg, soft, clock, acq, &ctx)) return false;
     std::vector<float> psd(files.size() * (size_t)nfft);
     dabb_survey_io sio; memset(&sio, 0, sizeof sio);
     sio.in = buf.data(); sio.in_is_host = 1; sio.iq_format = fmt; sio.in_stride = in_len; sio.n_inputs = (int32_t)files.size(); sio.nfft = nfft;
@@ -416,7 +429,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
         const int S = (int)cs.size();
         if (S == 0) return true;
         cfg.n_streams = S; cfg.disable_coarse = disable_coarse; cfg.freqsync_method = freqsync;
-        if (!create_scan_ctx(cfg, soft, clock, &ctx)) return false;
+        if (!create_scan_ctx(cfg, soft, clock, acq, &ctx)) return false;
         dabb_stream_reset(ctx, 0, S, 0);
         Outputs o; o.res.resize((size_t)S); o.fibs.resize((size_t)S * 12 * 32);
         std::vector<int64_t> buf_start((size_t)S);
@@ -485,7 +498,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
 
 int main(int argc, char** argv)
 {
-    int fmt = DABB_IQ_CF32, device = 0, soft = DABB_DEMAP_REFERENCE, clock = DABB_CLOCK_OFF; bool coarse = false, tii = false, ber = false; std::string out;
+    int fmt = DABB_IQ_CF32, device = 0, soft = DABB_DEMAP_REFERENCE, clock = DABB_CLOCK_OFF, acq = DABB_ACQ_REFERENCE; bool coarse = false, tii = false, ber = false; std::string out;
     int64_t rate = 0; std::vector<int64_t> offsets; bool scan_only = false, auto_offsets = false; int diversity = 0; bool diversity_set = false;
     std::vector<std::string> files;
     for (int i = 1; i < argc; i++) {
@@ -507,6 +520,11 @@ int main(int argc, char** argv)
             soft = m == "reference" ? DABB_DEMAP_REFERENCE : m == "weighted" ? DABB_DEMAP_WEIGHTED : -1;
             if (soft < 0) { fprintf(stderr, "unknown soft demap %s\n", m.c_str()); return 2; }
         }
+        else if (a == "--acq" && i + 1 < argc) {
+            const std::string m = argv[++i];
+            acq = m == "reference" ? DABB_ACQ_REFERENCE : m == "robust" ? DABB_ACQ_ROBUST : -1;
+            if (acq < 0) { fprintf(stderr, "unknown acquisition %s\n", m.c_str()); return 2; }
+        }
         else if (a == "--rate" && i + 1 < argc) rate = atoll(argv[++i]);
         else if (a == "--scan") scan_only = true;
         else if (a == "--offset" && i + 1 < argc && std::string(argv[i + 1]) == "auto") { auto_offsets = true; i++; }
@@ -522,7 +540,7 @@ int main(int argc, char** argv)
     }
     if (out.empty() || files.empty() || (rate > 0) != ((int)!offsets.empty() + (int)scan_only + (int)auto_offsets == 1)
         || (rate <= 0 && (scan_only || auto_offsets))) {
-        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock] [--diversity N] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
+        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock] [--acq robust|reference] [--diversity N] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
         return 2;
     }
     if (diversity_set && (rate > 0 || diversity < 1 || diversity > DABB_MAX_BRANCHES || files.size() % (size_t)diversity)) {
@@ -534,7 +552,7 @@ int main(int argc, char** argv)
     std::vector<std::vector<int64_t>> file_offsets(wide ? files.size() : 0, offsets);
     if (scan_only || auto_offsets) {
         std::vector<std::vector<Stream>> found;
-        if (!scan(files, rate, fmt, device, soft, clock, found)) return 1;
+        if (!scan(files, rate, fmt, device, soft, clock, acq, found)) return 1;
         for (size_t f = 0; f < files.size(); f++) {
             file_offsets[f].clear();
             for (const Stream& z : found[f]) file_offsets[f].push_back(z.offset + z.corr);
@@ -568,9 +586,10 @@ int main(int argc, char** argv)
     cfg.disable_coarse = coarse ? 0 : 1; cfg.n_subch_slots = DABB_MAX_SUBCH; cfg.max_subch_cu = 416;
     dabb_ctx* ctx = nullptr;
     if (dabb_create(&cfg, &ctx) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(nullptr)); return 1; }
-    if (tii || ber || soft != DABB_DEMAP_REFERENCE || clock != DABB_CLOCK_OFF) {
+    if (tii || ber || soft != DABB_DEMAP_REFERENCE || clock != DABB_CLOCK_OFF || acq != DABB_ACQ_REFERENCE) {
         dabb_options op; memset(&op, 0, sizeof op);
         op.disable_coarse = cfg.disable_coarse; op.decode_tii = tii; op.count_bit_errors = ber; op.soft_demap = soft; op.sample_clock = clock;
+        op.acquisition = acq;
         if (dabb_set_options(ctx, &op) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
     }
     if (diversity > 1) {          /* the antennas of one capture: the first file of each run of `diversity` leads */
@@ -601,7 +620,8 @@ int main(int argc, char** argv)
         if (clock) z.clk = fopen((out + "/" + z.name + ".clk").c_str(), "w");
         const bool leads = diversity > 1 && s % diversity == 0;
         if (leads) z.div = fopen((out + "/" + z.name + ".div").c_str(), "w");
-        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii) || (ber && !z.ber) || (clock && !z.clk) || (leads && !z.div)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
+        if (acq == DABB_ACQ_ROBUST) z.acq = fopen((out + "/" + z.name + ".acq").c_str(), "w");
+        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii) || (ber && !z.ber) || (clock && !z.clk) || (leads && !z.div) || (acq == DABB_ACQ_ROBUST && !z.acq)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
         z.acq_need = 3 * TF;
     }
     dabb_stream_reset(ctx, 0, S, 0);
@@ -609,6 +629,7 @@ int main(int argc, char** argv)
     Outputs o;
     o.res.resize((size_t)S); o.fibs.resize((size_t)S * 12 * 32); o.msc.resize((size_t)S * DABB_MAX_SUBCH * 4 * 1152); o.sf.resize((size_t)S * DABB_MAX_SUBCH * 5760);
     o.tres.resize(tii ? (size_t)S : 0); o.bres.resize(ber ? (size_t)S : 0); o.cres.resize(clock ? (size_t)S : 0); o.dres.resize(diversity > 1 ? (size_t)S : 0);
+    o.ares.resize(acq == DABB_ACQ_ROBUST ? (size_t)S : 0);
     std::vector<int64_t> buf_start((size_t)S);
 
     int active = S;
@@ -666,7 +687,7 @@ int main(int argc, char** argv)
     for (auto& z : st) {
         printf("%s frames=%ld fibs=%ld fib_crc_ok=%ld service=0x%X bitrate=%d logical_frames=%ld\n", z.name.c_str(), z.frames, z.fibs, z.fibs_ok, z.sid, z.bitrate, z.logical);
         if (z.in) fclose(z.in);
-        fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii); if (z.ber) fclose(z.ber); if (z.clk) fclose(z.clk); if (z.div) fclose(z.div);
+        fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii); if (z.ber) fclose(z.ber); if (z.clk) fclose(z.clk); if (z.div) fclose(z.div); if (z.acq) fclose(z.acq);
     }
     dabb_destroy(ctx);
     return 0;
