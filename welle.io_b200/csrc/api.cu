@@ -34,8 +34,6 @@ struct StreamState {
 
 struct StepScratch {        // per stream, rewritten every step
     int64_t win_start;      // T_u window for findIndex, relative to the stream buffer
-    int64_t prs_start;
-    int32_t nco_sync[2];
     int32_t nco_frame[4];
     int32_t active;         // this stream decodes a frame in this step
     int32_t status;
@@ -86,20 +84,41 @@ struct StepOut {
     dabb_frame_result* results; uint8_t* fibs; uint8_t* msc; int64_t msc_stride; uint8_t* sf; int64_t sf_stride;
 };
 
+// The optional analyses.  Each holds all its device buffers, is built whole when it is first enabled (a failed build leaves the context
+// without it) and lives until dabb_destroy; `res` is its tap's records of the last step.
+// TII (tii.cu): the null symbol when keep_taps has no tap for it, the spectra (tap 4), each stream's open combinations and their
+// phase-error sums, the step's analyses and the tie-order tables
+struct Tii {
+    DevBuf<float2> null, spectra; DevBuf<dabb_tii::StreamHdr> hdr; DevBuf<dabb_tii::Job> jobs; DevBuf<int32_t> njobs;
+    DevBuf<uint32_t> sums; DevBuf<uint16_t> rank; DevBuf<dabb_tii_result> res;
+};
+// channel bit-error count (ber.cu): the puncturing of every protection profile, then of the FIC, as the count reads it
+struct Ber { DevBuf<dabb_ber::Profile> prof; DevBuf<dabb_ber_result> res; };
+// sample-clock tracking: [2][S] the ppm each frame of a step is derotated with, double buffered by step parity like the other scratch
+struct Clock { DevBuf<float> frame; DevBuf<dabb_clock_result> res; };
+// robust acquisition (acq.cu): the cosine table of the block transform, each stream's search span, the block levels and envelope sums
+// [S][NB_MAX], the bins the excising find_index instance zeroed [S] (tap 13's `excised`, merged when it is read)
+struct Acq { DevBuf<float> cos, level, l1; DevBuf<AcqJob> job; DevBuf<int32_t> exc; DevBuf<dabb_acq_result> res; };
+// diversity combining (combine.cu): the tables of one grouping, built whole by rebuild_comb.  Per group its members and their r1 rows
+// (groups) and the (group, symbol) items of combine_kernel; per stream its group or -1 (gid).  Without keep_taps the OFDM kernel stores
+// the grouped streams' r1 of their leader's symbols in r1 (row[s], the symbols lmask[s] marks); with it combine_kernel reads tap 2.
+struct CombTables {
+    std::shared_ptr<const std::vector<int32_t>> leader;     // the leader table they were built from
+    int n_items = 0;
+    DevBuf<CombGroup> groups; DevBuf<CombItem> items; DevBuf<int32_t> gid, row; DevBuf<uint32_t> lmask; DevBuf<float2> r1;
+};
+// tab: the current grouping, null while no group of two or more exists
+struct Combining { DevBuf<dabb_combine_result> res; std::unique_ptr<CombTables> tab; };
+
 } // namespace
 
 struct dabb_ctx {
     int device = 0; cudaStream_t stream = nullptr; cudaStream_t streamB = nullptr; cudaEvent_t evA[2] = {nullptr, nullptr}, evB[2] = {nullptr, nullptr}; bool evB_valid[2] = {false, false};
     int64_t step = 0; int last_parity = 0; DevBuf<int32_t> d_fic_ratio, d_coarse;
     cudaStream_t stream2 = nullptr; cudaEvent_t ev_ofdm = nullptr, ev_fic = nullptr; DevBuf<uint2> d_dec_fic; int S = 0; int fft_mode = 0; int disable_coarse = 0; int keep_taps = 0; int placement = 0; int freqsync = 0;
-    int decode_tii = 0; DevBuf<float2> d_tii;
-    // TII analysis (tii.cu), allocated when decode_tii is first set: the null symbol when keep_taps has no tap for it, each stream's open
-    // combinations and their phase-error sums, the step's analyses, the tie-order tables and the step's records (tap 9)
-    DevBuf<float2> d_tii_null; DevBuf<dabb_tii::StreamHdr> d_tii_hdr; DevBuf<dabb_tii::Job> d_tii_jobs; DevBuf<int32_t> d_tii_njobs;
-    DevBuf<uint32_t> d_tii_sums; DevBuf<uint16_t> d_tii_rank; DevBuf<dabb_tii_result> d_tii_res;
-    // channel bit-error count (ber.cu), allocated when count_bit_errors is first set: the puncturing of every protection profile and of the
-    // FIC as the count reads it ([DABB_MAX_PROFILES] then the FIC) and the step's records (tap 10)
-    int count_ber = 0; dabb_ber::Profile h_ber_fic{}; DevBuf<dabb_ber::Profile> d_ber_prof; DevBuf<dabb_ber_result> d_ber_res;
+    // the optional analyses, null until first enabled, and the options that run them in a step (combining runs while comb->tab exists)
+    std::unique_ptr<Tii> tii; std::unique_ptr<Ber> ber; std::unique_ptr<Clock> clock; std::unique_ptr<Acq> acq; std::unique_ptr<Combining> comb;
+    int decode_tii = 0, count_ber = 0, sample_clock = DABB_CLOCK_OFF, acquisition = DABB_ACQ_REFERENCE;
     TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0;
     DevBuf<unsigned long long> d_trace_rec; DevBuf<unsigned int> d_trace_count;      // what `trace` points into
     std::string err; int64_t launches = 0; int osc_mismatches = -1; int osc_patched = 0; std::vector<float2> h_osc;
@@ -145,9 +164,6 @@ struct dabb_ctx {
     } pend[2], pend_sync;     // the two dabb_submit slots; dabb_process and taps 7 / 8, which never leave a step outstanding
     int pend_head = 0, pend_count = 0; int64_t submits = 0;
     int groups = 1; int fc_pitch = 1; int tail_frames = 0; int nco_fast = 0; int soft_demap = DABB_DEMAP_REFERENCE;
-    // sample-clock tracking, allocated when sample_clock is first set to TRACK: [2][S] the ppm each frame of a step is derotated with
-    // (double buffered by step parity, like the other per-step scratch) and the step's records (tap 11)
-    int sample_clock = DABB_CLOCK_OFF; DevBuf<float> d_clock_frame; DevBuf<dabb_clock_result> d_clock_res;
     DevBuf<const int32_t*> d_info_tab;
     // optional per-kernel timing: one event after every launch, durations = differences of consecutive events
     bool prof = false; std::vector<cudaEvent_t> prof_ev; std::vector<const char*> prof_name; size_t prof_used = 0;
@@ -157,23 +173,9 @@ struct dabb_ctx {
     // without keep_taps: [S][OFDM_MASK_WORDS] the OFDM symbols each stream's decoders read (ofdm_mask.cuh), rebuilt by every select and
     // remove call; the OFDM launch of the last step, which tap 0 repeats over every symbol when soft_partial says it skipped some
     DevBuf<uint32_t> d_symmask; OfdmParams soft_op{}; bool soft_partial = false;
-    // diversity combining (dabb_set_combining, combine.cu), all empty until a group of two or more forms (comb_on): the leader table; per
-    // group its members and their r1 rows (d_comb_groups) and the (group, symbol) items of combine_kernel (d_comb_items); per stream its
-    // group or -1 (d_comb_gid).  Without keep_taps the OFDM kernel stores the grouped streams' r1 of their leader's symbols in d_comb_r1
-    // (row d_comb_row[s], the symbols d_comb_lmask[s] marks); with it combine_kernel reads tap 2's d_r1.  d_comb_res: tap 12, kept once
-    // allocated.  The tap-0 repeat of the last step: comb_op, that step's combine launch (n_items 0: it had no group), and the grouping it
-    // ran with, the rows of every symbol (d_comb_groups_full, d_comb_row_full, comb_n_groups groups of comb_n_grouped streams in all).  A
-    // regroup stages the new grouping's (the *_next members, comb_staged) and the next step takes them over, so that tap 0 of the step
-    // before the regroup stays combined
-    std::vector<int32_t> h_leader; bool comb_on = false; int comb_n_groups = 0, comb_n_items = 0, comb_n_grouped = 0;
-    DevBuf<CombGroup> d_comb_groups, d_comb_groups_full; DevBuf<CombItem> d_comb_items; DevBuf<int32_t> d_comb_gid, d_comb_row, d_comb_row_full;
-    DevBuf<uint32_t> d_comb_lmask; DevBuf<float2> d_comb_r1; DevBuf<dabb_combine_result> d_comb_res; CombParams comb_op{};
-    DevBuf<CombGroup> d_comb_groups_next; DevBuf<int32_t> d_comb_row_next; int comb_next_groups = 0, comb_next_grouped = 0; bool comb_staged = false;
-    // robust acquisition (acquisition = DABB_ACQ_ROBUST, acq.cu), allocated when the option is first set: the cosine table of the block
-    // transform, each stream's search span, the block levels and envelope sums [S][NB_MAX], the bins the excising find_index instance
-    // zeroed [S], and the step's records (tap 13, with `excised` taken from d_acq_exc when it is read)
-    int acquisition = DABB_ACQ_REFERENCE; DevBuf<float> d_acq_cos, d_acq_level, d_acq_l1; DevBuf<AcqJob> d_acq_job; DevBuf<int32_t> d_acq_exc;
-    DevBuf<dabb_acq_result> d_acq_res;
+    // the combine launch of the last step (n_items 0: it had no group) and the leader table it ran with, from which tap 0 builds the rows
+    // of every symbol when it repeats that step, whatever grouping has replaced it since
+    CombParams comb_op{}; std::shared_ptr<const std::vector<int32_t>> comb_leader;
 };
 
 namespace {
@@ -195,6 +197,24 @@ template <typename T> int dalloc(dabb_ctx* ctx, DevBuf<T>& b, size_t n, bool zer
     if (!rc && zero) cudaMemsetAsync(b.get(), 0, n * sizeof(T), ctx->stream);
     return rc;
 }
+
+// an analysis's records of a step that did not run it: zeros
+template <typename T> int clear_records(dabb_ctx* ctx, const DevBuf<T>& res, cudaStream_t st)
+{
+    CK(cudaMemsetAsync(res, 0, sizeof(T) * ctx->S, st));
+    return DABB_OK;
+}
+
+// the S records of an analysis's last step into `out` (at most `bytes`); refused while it was never enabled
+template <typename A> int read_records(dabb_ctx* ctx, const std::unique_ptr<A>& a, const char* refusal, void* out, size_t bytes)
+{
+    if (!a) { ctx->err = refusal; return DABB_E_STATE; }
+    const size_t n = sizeof(*a->res.get()) * ctx->S;
+    CK(cudaMemcpy(out, a->res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost));
+    return DABB_OK;
+}
+
+CombTables* comb_tab(const dabb_ctx* ctx) { return ctx->comb ? ctx->comb->tab.get() : nullptr; }
 
 void prof_mark(dabb_ctx* ctx, const char* what)
 {
@@ -364,17 +384,18 @@ __global__ void plan_kernel(StreamState* st, StepScratch* scr, const int64_t* bu
     if (s >= S) return;
     const StreamState z = st[s];
     StepScratch c{};
+    int32_t lp = 0, p1 = 0;
     const int64_t rel = z.pos - buf_start[s];
     const int64_t need = (int64_t)TU + (TU - 1) + 75 * (int64_t)TS + TNULL;
     if (!z.acquired) { c.active = 0; c.status = DABB_FRAME_ACQUIRING; }
     else if (rel < 0 || rel + need > buf_len) { c.active = 0; c.status = DABB_FRAME_NEED_SAMPLES; }
     else {
         c.active = 1; c.status = DABB_FRAME_DECODED; c.win_start = rel;
-        const int32_t p1 = z.coarse + z.fine;
-        c.nco_sync[0] = mod_rate((int64_t)z.local_phase - p1); c.nco_sync[1] = p1;
+        p1 = z.coarse + z.fine;
+        lp = mod_rate((int64_t)z.local_phase - p1);
     }
     scr[s] = c;
-    win[s] = c.win_start; nco_sync[2 * s] = c.nco_sync[0]; nco_sync[2 * s + 1] = c.nco_sync[1]; active[s] = c.active;
+    win[s] = c.win_start; nco_sync[2 * s] = lp; nco_sync[2 * s + 1] = p1; active[s] = c.active;
 }
 
 // clock_frame (DABB_CLOCK_TRACK, else nullptr): the ppm the OFDM kernel derotates the frame with, the estimate from before the frame
@@ -396,7 +417,6 @@ __global__ void post_sync_kernel(StreamState* st, StepScratch* scr, const int32_
         st[s] = z; scr[s] = c; active[s] = 0;
         return;
     }
-    c.prs_start = c.win_start + idx;
     // phase applied to PRS sample 0 (the (idx+1)-th sample read in this frame)
     const int32_t lp_prs0 = mod_rate((int64_t)z.local_phase - (int64_t)(idx + 1) * p1);
     // coarse corrector (ofdm-processor.cpp:397-409): find_index_kernel evaluated processPRS where the FIC ratio asked for it
@@ -410,7 +430,7 @@ __global__ void post_sync_kernel(StreamState* st, StepScratch* scr, const int32_
     const int32_t lp_sym0 = mod_rate((int64_t)lp_after_prs - p2 + (int64_t)TU * p2);   // so that lp(i) = lp_sym0 - i*p2 for i >= 2048
     c.nco_frame[0] = lp_prs0; c.nco_frame[1] = p1; c.nco_frame[2] = lp_sym0; c.nco_frame[3] = p2;
     scr[s] = c; st[s] = z;
-    prs[s] = c.prs_start;
+    prs[s] = c.win_start + idx;
     nco_frame[4 * s] = lp_prs0; nco_frame[4 * s + 1] = p1; nco_frame[4 * s + 2] = lp_sym0; nco_frame[4 * s + 3] = p2;
     if (clock_frame) clock_frame[s] = (float)dabb_clock::applied(z.clk);
 }
@@ -588,6 +608,21 @@ __global__ void convert_iq_kernel(const uint8_t* __restrict__ raw, int64_t raw_s
     out[(int64_t)s * out_stride + i] = make_float2(v.x, v.y);
 }
 
+// an analysis switched on (`on`) for the first time: `build` fills a new instance, which the context takes only when every allocation and
+// upload succeeded
+template <typename A, typename F> int enable(dabb_ctx* ctx, bool on, std::unique_ptr<A>& owner, F build)
+{
+    if (!on || owner) return DABB_OK;
+    cudaSetDevice(ctx->device);
+    sync_all(ctx);
+    auto a = std::make_unique<A>();
+    int rc;
+    if ((rc = build(*a))) return rc;
+    CK(cudaStreamSynchronize(ctx->stream));
+    owner = std::move(a);
+    return DABB_OK;
+}
+
 // makes b hold at least n elements, without keeping its contents; the device finishes with the old buffer first
 template <typename T> int grow(dabb_ctx* ctx, DevBuf<T>& b, size_t n)
 {
@@ -702,7 +737,7 @@ int add_profile(dabb_ctx* ctx, const ProtProfile& prof)
     CK(cudaMemcpyAsync(pf.d_prbs_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_profiles + ctx->profiles.size(), &e, sizeof e, cudaMemcpyHostToDevice, ctx->stream));
     build_ber_profile(*ctx->host, prof.nblk, prof.L, prof.PI, pf.nbits, pf.ber); pf.ber.prbs = pf.d_prbs_words;
-    if (ctx->d_ber_prof) CK(cudaMemcpyAsync(ctx->d_ber_prof + ctx->profiles.size(), &pf.ber, sizeof pf.ber, cudaMemcpyHostToDevice, ctx->stream));
+    if (ctx->ber) CK(cudaMemcpyAsync(ctx->ber->prof + ctx->profiles.size(), &pf.ber, sizeof pf.ber, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     ctx->profiles.push_back(std::move(pf));
     return DABB_OK;
@@ -738,13 +773,14 @@ void own_symmask(dabb_ctx* ctx, int s, uint32_t* m)
 int upload_symmask(dabb_ctx* ctx, int first, int count)
 {
     if (!ctx->d_symmask) return DABB_OK;
-    if (ctx->comb_on) { first = 0; count = ctx->S; }
+    const CombTables* ct = comb_tab(ctx);
+    if (ct) { first = 0; count = ctx->S; }
     std::vector<uint32_t> m((size_t)count * OFDM_MASK_WORDS);
     for (int i = 0; i < count; i++) own_symmask(ctx, first + i, m.data() + (size_t)i * OFDM_MASK_WORDS);
-    if (ctx->comb_on) {
+    if (ct) {
         std::vector<uint32_t> own(m);
         for (int s = 0; s < ctx->S; s++) {
-            const int L = ctx->h_leader[(size_t)s];
+            const int L = (*ct->leader)[(size_t)s];
             for (int w = 0; w < OFDM_MASK_WORDS; w++) m[(size_t)s * OFDM_MASK_WORDS + w] |= own[(size_t)L * OFDM_MASK_WORDS + w];
         }
     }
@@ -760,69 +796,63 @@ template <typename T> int upload(dabb_ctx* ctx, DevBuf<T>& b, const std::vector<
     return DABB_OK;
 }
 
-// the tables of diversity combining from h_leader and the leaders' symbol masks (the caller has run sync_all).  Each group of two or more
-// streams combines the data symbols its leader's decoders read (every symbol with keep_taps); without keep_taps its members' r1 rows of
-// those symbols lie one after the other in d_comb_r1.  `regroup`: the grouping itself changed, so the rows of every symbol are staged for
-// the tap-0 repeat of the next step; the last step's stay for its own repeat.  No group: every table the next step would read is freed
-// (tap 12's records stay).
-int rebuild_comb(dabb_ctx* ctx, bool regroup)
+// every data symbol (1..75), as the mask of a group that combines them all
+void all_symbols(int, uint32_t* m) { for (int l = 1; l <= 75; l++) m[l >> 5] |= 1u << (l & 31); }
+
+// The groups of two or more streams that a leader table forms, in leader order with their members in stream order.  mask(L, m) marks the
+// data symbols the group of leader L combines: one item of combine_kernel each, and one r1 row each for every member, the members' rows
+// one after the other and the groups' too (`rows` in all).  Per stream its group (gid, -1: none), first row and its group's mask.
+struct Grouping { std::vector<CombGroup> groups; std::vector<CombItem> items; std::vector<int32_t> gid, row; std::vector<uint32_t> lmask; int64_t rows = 0; };
+template <typename F> Grouping group_streams(const std::vector<int32_t>& leader, F mask)
 {
-    const int S = ctx->S, W = OFDM_MASK_WORDS;
-    const bool taps = !ctx->d_symmask;
-    std::vector<std::vector<int32_t>> members(ctx->h_leader.empty() ? 0 : (size_t)S);
-    for (int s = 0; s < (int)members.size(); s++) members[(size_t)ctx->h_leader[(size_t)s]].push_back(s);
-    std::vector<CombGroup> groups, full; std::vector<CombItem> items;
-    std::vector<int32_t> gid((size_t)S, -1), row((size_t)S, -1), row_full((size_t)S, -1); std::vector<uint32_t> lmask((size_t)S * W, 0u);
-    int64_t rows = 0; int rank = 0;
-    for (int L = 0; L < (int)members.size(); L++) {
+    const int S = (int)leader.size(), W = OFDM_MASK_WORDS;
+    std::vector<std::vector<int32_t>> members((size_t)S);
+    for (int s = 0; s < S; s++) members[(size_t)leader[(size_t)s]].push_back(s);
+    Grouping gr;
+    gr.gid.assign((size_t)S, -1); gr.row.assign((size_t)S, -1); gr.lmask.assign((size_t)S * W, 0u);
+    for (int L = 0; L < S; L++) {
         const auto& mb = members[(size_t)L];
         if (mb.size() < 2) continue;
         uint32_t m[OFDM_MASK_WORDS] = {0u, 0u, 0u, 0u};
-        if (taps) for (int l = 1; l <= 75; l++) m[l >> 5] |= 1u << (l & 31);
-        else own_symmask(ctx, L, m);
+        mask(L, m);
+        const int gi = (int)gr.groups.size();
         int nsym = 0;
-        for (int w = 0; w < W; w++) for (uint32_t x = m[w]; x; x &= x - 1) nsym++;
-        CombGroup g{}, gf{};
-        g.n = gf.n = (int32_t)mb.size();
-        const int gi = (int)groups.size();
+        for (int l = 1; l <= 75; l++)
+            if ((m[l >> 5] >> (l & 31)) & 1u) { gr.items.push_back(CombItem{gi, l, nsym, nsym == 0}); nsym++; }
+        CombGroup g{};
+        g.n = (int32_t)mb.size();
         for (int i = 0; i < g.n; i++) {
             const int s = mb[(size_t)i];
-            if (s == L) g.lpos = gf.lpos = i;
-            g.stream[i] = gf.stream[i] = s;
-            g.row[i] = taps ? 75 * s : (int32_t)(rows + (int64_t)i * nsym);
-            gf.row[i] = 75 * (rank + i);
-            gid[(size_t)s] = gi; row[(size_t)s] = g.row[i]; row_full[(size_t)s] = gf.row[i];
-            for (int w = 0; w < W; w++) lmask[(size_t)s * W + w] = m[w];
+            if (s == L) g.lpos = i;
+            g.stream[i] = s; g.row[i] = (int32_t)(gr.rows + (int64_t)i * nsym);
+            gr.gid[(size_t)s] = gi; gr.row[(size_t)s] = g.row[i];
+            for (int w = 0; w < W; w++) gr.lmask[(size_t)s * W + w] = m[w];
         }
-        int col = 0;
-        for (int l = 1; l <= 75; l++)
-            if ((m[l >> 5] >> (l & 31)) & 1u) { items.push_back(CombItem{gi, l, taps ? l - 1 : col, col == 0}); col++; }
-        rows += (int64_t)g.n * nsym; rank += g.n;
-        groups.push_back(g); full.push_back(gf);
+        gr.rows += (int64_t)g.n * nsym;
+        gr.groups.push_back(g);
     }
-    ctx->comb_on = !groups.empty();
-    if (regroup) {
-        ctx->d_comb_groups_next.reset(); ctx->d_comb_row_next.reset();
-        ctx->comb_next_groups = ctx->comb_next_grouped = 0; ctx->comb_staged = true;
-    }
-    if (!ctx->comb_on) {
-        ctx->d_comb_groups.reset(); ctx->d_comb_items.reset(); ctx->d_comb_gid.reset(); ctx->d_comb_row.reset();
-        ctx->d_comb_lmask.reset(); ctx->d_comb_r1.reset();
-        ctx->comb_n_items = 0;
-        return DABB_OK;
-    }
+    return gr;
+}
+
+// The tables of diversity combining for a leader table that forms at least one group, built whole and then swapped into c (the caller
+// has run sync_all).  Each group combines the data symbols its leader's decoders read; with keep_taps every symbol, from tap 2's rows.
+// A failure leaves c's tables as they were: the last step, which cannot fail, takes over their r1 buffer when it is neither too small
+// nor more than twice the size needed.
+int rebuild_comb(dabb_ctx* ctx, Combining& c, std::shared_ptr<const std::vector<int32_t>> leader)
+{
+    const bool taps = !ctx->d_symmask;
+    Grouping gr = group_streams(*leader, [&](int L, uint32_t* m) { if (taps) all_symbols(L, m); else own_symmask(ctx, L, m); });
+    if (taps) for (CombGroup& g : gr.groups) for (int i = 0; i < g.n; i++) g.row[i] = 75 * g.stream[i];
+    auto t = std::make_unique<CombTables>();
+    t->leader = std::move(leader); t->n_items = (int)gr.items.size();
+    const size_t need = (size_t)gr.rows * KC;
+    const bool keep_r1 = !taps && c.tab && need <= c.tab->r1.size() && 2 * need >= c.tab->r1.size();
     int rc;
-    if ((rc = upload(ctx, ctx->d_comb_groups, groups)) || (rc = upload(ctx, ctx->d_comb_items, items)) || (rc = upload(ctx, ctx->d_comb_gid, gid))) return rc;
-    if (!taps) {
-        if ((rc = upload(ctx, ctx->d_comb_row, row)) || (rc = upload(ctx, ctx->d_comb_lmask, lmask))) return rc;
-        if ((size_t)rows * KC > ctx->d_comb_r1.size() || (size_t)rows * KC * 2 < ctx->d_comb_r1.size()) { ctx->d_comb_r1.reset(); if ((rc = alloc(ctx, ctx->d_comb_r1, (size_t)rows * KC))) return rc; }
-        if (regroup) {
-            if ((rc = upload(ctx, ctx->d_comb_groups_next, full)) || (rc = upload(ctx, ctx->d_comb_row_next, row_full))) return rc;
-            ctx->comb_next_groups = (int)groups.size(); ctx->comb_next_grouped = rank;
-        }
-    }
+    if ((rc = upload(ctx, t->groups, gr.groups)) || (rc = upload(ctx, t->items, gr.items)) || (rc = upload(ctx, t->gid, gr.gid))) return rc;
+    if (!taps && ((rc = upload(ctx, t->row, gr.row)) || (rc = upload(ctx, t->lmask, gr.lmask)) || (!keep_r1 && (rc = alloc(ctx, t->r1, need))))) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
-    ctx->comb_n_items = (int)items.size();
+    if (keep_r1) t->r1 = std::move(c.tab->r1);
+    c.tab = std::move(t);
     return DABB_OK;
 }
 
@@ -858,7 +888,7 @@ int set_slot_streams(dabb_ctx* ctx, int slot, int first, int count, const MscSlo
     }
     set_slot_kernel<<<(count + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_slots, ns, slot, first, count, v);
     for (int i = first; i < first + count; i++) ctx->h_slots[(size_t)i * ns + slot] = v;
-    if ((rc = upload_symmask(ctx, first, count)) || (ctx->comb_on && (rc = rebuild_comb(ctx, false)))) return rc;
+    if ((rc = upload_symmask(ctx, first, count)) || (comb_tab(ctx) && (rc = rebuild_comb(ctx, *ctx->comb, comb_tab(ctx)->leader)))) return rc;
     { int rc_ = check_launch(ctx, "set_slot_kernel"); cudaStreamSynchronize(ctx->stream); return rc_; }
 }
 
@@ -945,8 +975,6 @@ int dabb_create(const dabb_config* cfg, dabb_ctx** out)
         std::vector<uint32_t> w(768 / 32); build_prbs_words(768, w.data());
         if ((rc = dalloc(ctx, ctx->d_fic_prbs_words, w.size()))) return fail(rc);
         cudaMemcpy(ctx->d_fic_prbs_words, w.data(), w.size() * 4, cudaMemcpyHostToDevice);
-        const int fic_L[2] = {21, 3}, fic_PI[2] = {16, 15};
-        build_ber_profile(*ctx->host, 2, fic_L, fic_PI, 768, ctx->h_ber_fic); ctx->h_ber_fic.prbs = ctx->d_fic_prbs_words;
         // expansion tables of the decoder kernel for the FIC puncturing (fic-handler.cpp:144-191)
         std::vector<uint2> steps; std::vector<uint32_t> soff;
         build_vit_tables_u2(ctx->host->fic_map, 774, steps, soff);
@@ -1036,7 +1064,7 @@ int dabb_stream_reset(dabb_ctx* ctx, int32_t first, int32_t count, int64_t pos)
     cudaSetDevice(ctx->device);
     sync_all(ctx);
     reset_kernel<<<(count + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_state, ctx->d_slots, ctx->n_slots, first, count, pos, ctx->d_fic_ratio);
-    if (ctx->d_tii_hdr) CK(cudaMemsetAsync(ctx->d_tii_hdr + first, 0, sizeof(dabb_tii::StreamHdr) * count, ctx->stream));     // no open TII combinations
+    if (ctx->tii) CK(cudaMemsetAsync(ctx->tii->hdr + first, 0, sizeof(dabb_tii::StreamHdr) * count, ctx->stream));     // no open TII combinations
     for (int i = first; i < first + count; i++) for (int k = 0; k < ctx->n_slots; k++) { ctx->h_slots[(size_t)i * ctx->n_slots + k].cif_count = 0; ctx->h_slots[(size_t)i * ctx->n_slots + k].sf_frame_count = 0; }
     { int rc_ = check_launch(ctx, "reset_kernel"); cudaStreamSynchronize(ctx->stream); ctx->evB_valid[0] = ctx->evB_valid[1] = false; return rc_; }
 }
@@ -1095,7 +1123,7 @@ int dabb_set_combining(dabb_ctx* ctx, const int32_t* leader, int32_t n)
 {
     if (!ctx) return DABB_E_ARG;
     const int S = ctx->S;
-    std::vector<int32_t> L((size_t)S);
+    bool grouped = false;       // some stream is not its own leader: a group of two or more forms
     if (leader) {
         if (n != S) { ctx->err = "dabb_set_combining: the table needs n_streams entries"; return DABB_E_ARG; }
         std::vector<int> size((size_t)S, 0);
@@ -1104,18 +1132,22 @@ int dabb_set_combining(dabb_ctx* ctx, const int32_t* leader, int32_t n)
             if (v < 0 || v >= S) { ctx->err = "dabb_set_combining: leader[" + std::to_string(s) + "] is not a stream"; return DABB_E_ARG; }
             if (leader[v] != v) { ctx->err = "dabb_set_combining: leader[" + std::to_string(s) + "] is not a leader (leader[leader[s]] != leader[s])"; return DABB_E_ARG; }
             if (++size[(size_t)v] > DABB_MAX_BRANCHES) { ctx->err = "dabb_set_combining: a group has more than DABB_MAX_BRANCHES members"; return DABB_E_ARG; }
-            L[(size_t)s] = v;
+            grouped |= v != s;
         }
-    } else
-        for (int s = 0; s < S; s++) L[(size_t)s] = s;
+    }
     cudaSetDevice(ctx->device);
     sync_all(ctx);
-    const bool was = ctx->comb_on;
-    ctx->h_leader = L;
+    const bool was = comb_tab(ctx) != nullptr;
     int rc;
-    if ((rc = rebuild_comb(ctx, true))) return rc;
-    if (ctx->comb_on && !ctx->d_comb_res && (rc = dalloc(ctx, ctx->d_comb_res, (size_t)S))) return rc;
-    if ((was || ctx->comb_on) && (rc = upload_symmask(ctx, 0, S))) return rc;
+    if (grouped) {
+        // a group of two or more: its tables, with tap 12's records when this is the first group the context forms
+        std::unique_ptr<Combining> fresh;
+        if (!ctx->comb) { fresh = std::make_unique<Combining>(); if ((rc = dalloc(ctx, fresh->res, (size_t)S))) return rc; }
+        if ((rc = rebuild_comb(ctx, fresh ? *fresh : *ctx->comb, std::make_shared<const std::vector<int32_t>>(leader, leader + S)))) return rc;
+        if (fresh) ctx->comb = std::move(fresh);
+    } else if (ctx->comb)
+        ctx->comb->tab = nullptr;       // no group: every table is freed, tap 12's records stay
+    if ((was || comb_tab(ctx)) && (rc = upload_symmask(ctx, 0, S))) return rc;
     CK(cudaStreamSynchronize(ctx->stream));
     return DABB_OK;
 }
@@ -1207,19 +1239,17 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     const int tb = 128, gb = (S + tb - 1) / tb;
     // ---------------- lane A
     const bool robust = ctx->acquisition == DABB_ACQ_ROBUST;
+    Acq* aq = ctx->acq.get();
     if (robust) {       // the spectral null search of every stream that is not tracking, then the same hand-off to time sync
-        CK(cudaMemsetAsync(ctx->d_acq_exc, 0, sizeof(int32_t) * S, A));
-        acq_plan_kernel<<<gb, tb, 0, A>>>(ctx->d_state, ctx->d_buf_start, io->buf_len, S, ctx->d_acq_job);
+        if ((rc = clear_records(ctx, aq->exc, A))) return rc;
+        acq_plan_kernel<<<gb, tb, 0, A>>>(ctx->d_state, ctx->d_buf_start, io->buf_len, S, aq->job);
         if ((rc = check_launch(ctx, "acq_plan_kernel"))) return rc;
-        launch_acq_levels(ctx->d_acq_job, iq, stride, ctx->dev.osc, ctx->d_acq_cos, S, ctx->d_acq_level, ctx->d_acq_l1, A);
+        launch_acq_levels(aq->job, iq, stride, ctx->dev.osc, aq->cos, S, aq->level, aq->l1, A);
         if ((rc = check_launch(ctx, "acq_level_kernel"))) return rc;
-        acq_decide_kernel<<<S, 256, 0, A>>>(ctx->d_state, ctx->d_acq_job, ctx->d_buf_start, ctx->d_acq_level, ctx->d_acq_l1, ctx->d_acq_res);
+        acq_decide_kernel<<<S, 256, 0, A>>>(ctx->d_state, aq->job, ctx->d_buf_start, aq->level, aq->l1, aq->res);
         if ((rc = check_launch(ctx, "acq_decide_kernel"))) return rc;
     } else {
-        if (ctx->d_acq_res) {     // tap 13: nothing searched robustly in this step
-            CK(cudaMemsetAsync(ctx->d_acq_res, 0, sizeof(dabb_acq_result) * S, A));
-            CK(cudaMemsetAsync(ctx->d_acq_exc, 0, sizeof(int32_t) * S, A));
-        }
+        if (aq && ((rc = clear_records(ctx, aq->res, A)) || (rc = clear_records(ctx, aq->exc, A)))) return rc;     // tap 13: nothing searched robustly
         acquire_kernel<<<(S + 31) / 32, 32, 0, A>>>(ctx->d_state, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, S);
         if ((rc = check_launch(ctx, "acquire_kernel"))) return rc;
     }
@@ -1228,7 +1258,7 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     SyncParams sp{}; sp.iq = iq; sp.stride = stride; sp.win_start = d_win; sp.nco = d_nco_sync; sp.active = d_active; sp.index_out = d_index; sp.cir_out = ctx->d_cir; sp.n = S;
     sp.fic_ratio = ctx->d_fic_ratio; sp.coarse_out = ctx->disable_coarse ? nullptr : ctx->d_coarse.get(); sp.placement = ctx->placement; sp.freqsync = ctx->freqsync;
     sp.cir_work = ctx->d_cir_work;
-    launch_find_index(ctx->dev, sp, A, 0, robust ? ctx->d_acq_exc.get() : nullptr);
+    launch_find_index(ctx->dev, sp, A, 0, robust ? aq->exc.get() : nullptr);
     if ((rc = check_launch(ctx, robust ? "find_index_excise_kernel" : "find_index_kernel"))) return rc;
     launch_find_index(ctx->dev, sp, A, 1);
     if ((rc = check_launch(ctx, "find_search_kernel"))) return rc;
@@ -1237,55 +1267,52 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
         if ((rc = check_launch(ctx, "find_coarse_kernel"))) return rc;
     }
     const bool track = ctx->sample_clock == DABB_CLOCK_TRACK;
-    float* d_clock_frame = track ? ctx->d_clock_frame + (size_t)par * S : nullptr;
+    float* d_clock_frame = track ? ctx->clock->frame + (size_t)par * S : nullptr;
     post_sync_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, d_index, ctx->disable_coarse ? nullptr : ctx->d_coarse.get(), S, d_prs, d_nco_frame, d_active, d_clock_frame);
     if ((rc = check_launch(ctx, "post_sync_kernel"))) return rc;
+    const CombTables* ct = comb_tab(ctx);
     OfdmParams op{}; op.iq = iq; op.stride = stride; op.prs_start = d_prs; op.nco = d_nco_frame; op.active = d_active; op.soft = d_soft; op.soft_stride = DABB_SOFT_PER_FRAME;
     op.r1 = ctx->d_r1; op.freqcorr = d_fc; op.level = d_lvl; op.snr = d_snr; op.n_frames = S; op.groups = ctx->groups; op.sym_per_cta = 75 / ctx->groups;
     op.trace = ctx->trace;
     op.n_full = S - ctx->tail_frames; op.tail_groups = ctx->tail_frames ? OFDM_TAIL_GROUPS : 1; op.fc_pitch = ctx->fc_pitch; op.nco_fast = ctx->nco_fast; op.weighted = ctx->soft_demap == DABB_DEMAP_WEIGHTED;
     op.symmask = ctx->d_symmask; op.clock = d_clock_frame;
-    if (ctx->comb_on && !ctx->keep_taps) { op.r1 = ctx->d_comb_r1; op.r1_row = ctx->d_comb_row; op.r1_lmask = ctx->d_comb_lmask; }     // the grouped streams' r1 of their leader's symbols
+    if (ct && !ctx->keep_taps) { op.r1 = ct->r1; op.r1_row = ct->row; op.r1_lmask = ct->lmask; }     // the grouped streams' r1 of their leader's symbols
     launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, A);
     ctx->soft_op = op; ctx->soft_partial = op.symmask != nullptr;
     if ((rc = check_launch(ctx, "ofdm_demod_kernel"))) return rc;
-    advance_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, S, ctx->fc_pitch, d_fc, d_lvl, track, ctx->d_clock_res.get());
+    advance_kernel<<<gb, tb, 0, A>>>(ctx->d_state, scr, S, ctx->fc_pitch, d_fc, d_lvl, track, ctx->clock ? ctx->clock->res.get() : nullptr);
     if ((rc = check_launch(ctx, "advance_kernel"))) return rc;
     // the null symbol: tap 3 with keep_taps, else (TII only) an internal buffer
-    float2* d_null = ctx->d_null ? ctx->d_null.get() : (ctx->decode_tii ? ctx->d_tii_null.get() : nullptr);
+    Tii* tii = ctx->decode_tii ? ctx->tii.get() : nullptr;
+    float2* d_null = ctx->d_null ? ctx->d_null.get() : (tii ? tii->null.get() : nullptr);
     if (d_null) {
         null_tap_kernel<<<S, 256, 0, A>>>(scr, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, d_null);
         if ((rc = check_launch(ctx, "null_tap_kernel"))) return rc;
-        if (ctx->decode_tii) {
-            if (!ctx->d_tii && (rc = dalloc(ctx, ctx->d_tii, (size_t)S * 2 * TU))) return rc;
-            launch_tii_spectra(ctx->dev, iq, stride, d_prs, d_nco_frame, d_active, d_null, ctx->d_tii, S, A);
+        if (tii) {
+            launch_tii_spectra(ctx->dev, iq, stride, d_prs, d_nco_frame, d_active, d_null, tii->spectra, S, A);
             if ((rc = check_launch(ctx, "tii_spectra_kernel"))) return rc;
-            TiiParams tp{}; tp.spectra = ctx->d_tii; tp.active = d_active; tp.hdr = ctx->d_tii_hdr; tp.jobs = ctx->d_tii_jobs; tp.njobs = ctx->d_tii_njobs;
-            tp.sums = ctx->d_tii_sums; tp.rank = ctx->d_tii_rank; tp.res = ctx->d_tii_res.get(); tp.n = S;
+            TiiParams tp{}; tp.spectra = tii->spectra; tp.active = d_active; tp.hdr = tii->hdr; tp.jobs = tii->jobs; tp.njobs = tii->njobs;
+            tp.sums = tii->sums; tp.rank = tii->rank; tp.res = tii->res.get(); tp.n = S;
             launch_tii_plan(tp, A);
             if ((rc = check_launch(ctx, "tii_plan_kernel"))) return rc;
             launch_tii_phase(tp, A);
             if ((rc = check_launch(ctx, "tii_phase_kernel"))) return rc;
         }
     }
-    if (!ctx->decode_tii && ctx->d_tii_res) CK(cudaMemsetAsync(ctx->d_tii_res, 0, sizeof(dabb_tii_result) * S, A));     // tap 9: nothing analysed in this step
-    // diversity combining: the members' noise powers, then the leaders' softbits from their groups' products.  The tap-0 repeat of this
-    // step uses the grouping staged by a regroup since the last step
-    if (ctx->comb_staged) {
-        ctx->d_comb_groups_full = std::move(ctx->d_comb_groups_next); ctx->d_comb_row_full = std::move(ctx->d_comb_row_next);
-        ctx->comb_n_groups = ctx->comb_next_groups; ctx->comb_n_grouped = ctx->comb_next_grouped; ctx->comb_staged = false;
-    }
-    ctx->comb_op = CombParams{};
-    if (ctx->comb_on) {
-        null_power_kernel<<<S, dabb_comb::NULL_THREADS, 0, A>>>(scr, ctx->d_comb_gid, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, ctx->d_comb_res);
+    if (!tii && ctx->tii && (rc = clear_records(ctx, ctx->tii->res, A))) return rc;     // tap 9: nothing analysed in this step
+    // diversity combining: the members' noise powers, then the leaders' softbits from their groups' products.  The step's combine launch
+    // and leader table are kept for the tap-0 repeat.
+    ctx->comb_op = CombParams{}; ctx->comb_leader = nullptr;
+    if (ct) {
+        null_power_kernel<<<S, dabb_comb::NULL_THREADS, 0, A>>>(scr, ct->gid, iq, stride, ctx->d_buf_start, io->buf_len, ctx->dev.osc, ctx->comb->res);
         if ((rc = check_launch(ctx, "null_power_kernel"))) return rc;
-        CombParams cp{}; cp.groups = ctx->d_comb_groups; cp.items = ctx->d_comb_items; cp.n_items = ctx->comb_n_items; cp.r1 = ctx->keep_taps ? ctx->d_r1.get() : ctx->d_comb_r1.get();
-        cp.active = d_active; cp.prs = d_prs; cp.buf_start = ctx->d_buf_start; cp.res = ctx->d_comb_res.get(); cp.soft = d_soft; cp.soft_stride = DABB_SOFT_PER_FRAME;
+        CombParams cp{}; cp.groups = ct->groups; cp.items = ct->items; cp.n_items = ct->n_items; cp.r1 = ctx->keep_taps ? ctx->d_r1.get() : ct->r1.get();
+        cp.active = d_active; cp.prs = d_prs; cp.buf_start = ctx->d_buf_start; cp.res = ctx->comb->res.get(); cp.soft = d_soft; cp.soft_stride = DABB_SOFT_PER_FRAME;
         cp.weighted = ctx->soft_demap == DABB_DEMAP_WEIGHTED;
         launch_combine(cp, A);
         if ((rc = check_launch(ctx, "combine_kernel"))) return rc;
-        ctx->comb_op = cp;
-    } else if (ctx->d_comb_res) CK(cudaMemsetAsync(ctx->d_comb_res, 0, sizeof(dabb_combine_result) * S, A));     // tap 12: no group in this step
+        ctx->comb_op = cp; ctx->comb_leader = ct->leader;
+    } else if (ctx->comb && (rc = clear_records(ctx, ctx->comb->res, A))) return rc;     // tap 12: no group in this step
     if (!serial) { CK(cudaEventRecord(ctx->evA[par], A)); CK(cudaStreamWaitEvent(B, ctx->evA[par], 0)); }
     // ---------------- lane B: FIC chain forked onto its own stream, MSC chain per slot (longest first), then the result record.
     // (One fused Viterbi launch over FIC + MSC codewords was measured slower: 1.44 ms vs 0.34 + 1.02 ms.)
@@ -1326,10 +1353,10 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
             const auto& sl = ctx->slot[k];
             if (sl.configured) bp.slot[k] = BerSlot{sl.d_frag, sl.frag_pitch, sl.d_valid, sl.d_logical, sl.flen_pad};
         }
-        bp.profiles = ctx->d_ber_prof; bp.fic_profile = DABB_MAX_PROFILES; bp.res = ctx->d_ber_res.get(); bp.n_streams = S;
+        bp.profiles = ctx->ber->prof; bp.fic_profile = DABB_MAX_PROFILES; bp.res = ctx->ber->res.get(); bp.n_streams = S;
         launch_ber(bp, B);
         if ((rc = check_launch(ctx, "ber_kernel"))) return rc;
-    } else if (ctx->d_ber_res) CK(cudaMemsetAsync(ctx->d_ber_res, 0, sizeof(dabb_ber_result) * S, B));     // tap 10: nothing counted in this step
+    } else if (ctx->ber && (rc = clear_records(ctx, ctx->ber->res, B))) return rc;     // tap 10: nothing counted in this step
     CK(cudaMemcpyAsync((void*)ctx->d_info_tab, h_info, sizeof(void*) * DABB_MAX_SUBCH, cudaMemcpyHostToDevice, B));
     finalize_kernel<<<gb, tb, 0, B>>>(scr, ctx->d_slots, ctx->n_slots, S, ctx->d_fic_ratio, d_snr, ctx->d_crc, ctx->d_info_tab, ctx->d_results);
     if ((rc = check_launch(ctx, "finalize_kernel"))) return rc;
@@ -1460,18 +1487,20 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
         // per-frame parameters, writing nothing but the softbits (the symbols it did demap get the same bytes again)
         OfdmParams op = ctx->soft_op;
         op.symmask = nullptr; op.r1 = nullptr; op.r1_row = nullptr; op.r1_lmask = nullptr; op.freqcorr = nullptr; op.level = nullptr; op.snr = nullptr; op.trace = TraceBuf{nullptr, nullptr, 0};
-        // a step that combined: the grouped streams' r1 of every symbol into a temporary, then the combination over every symbol
-        DevBuf<float2> full;
-        const bool comb = ctx->comb_op.n_items > 0 && ctx->d_comb_groups_full;
+        // a step that combined: the grouped streams' r1 of every symbol into a temporary, then the combination over every symbol, with
+        // tables built from the leader table that step ran with (each member holds 75 rows, in group order)
+        const bool comb = ctx->comb_op.n_items > 0;
+        const Grouping gr = comb ? group_streams(*ctx->comb_leader, all_symbols) : Grouping{};
+        DevBuf<CombGroup> groups; DevBuf<int32_t> rows; DevBuf<float2> full;
         if (comb) {
             int rc;
-            if ((rc = alloc(ctx, full, (size_t)ctx->comb_n_grouped * 75 * KC))) return rc;
-            op.r1 = full; op.r1_row = ctx->d_comb_row_full;
+            if ((rc = upload(ctx, groups, gr.groups)) || (rc = upload(ctx, rows, gr.row)) || (rc = alloc(ctx, full, (size_t)gr.rows * KC))) return rc;
+            op.r1 = full; op.r1_row = rows;
         }
         launch_ofdm_demod(ctx->dev, op, ctx->fft_mode, ctx->stream);
         CK(cudaGetLastError());
         if (comb) {
-            CombParams cp = ctx->comb_op; cp.groups = ctx->d_comb_groups_full; cp.items = nullptr; cp.n_items = ctx->comb_n_groups * 75; cp.r1 = full;
+            CombParams cp = ctx->comb_op; cp.groups = groups; cp.items = nullptr; cp.n_items = (int)gr.groups.size() * 75; cp.r1 = full;
             launch_combine(cp, ctx->stream);
             CK(cudaGetLastError());
         }
@@ -1486,31 +1515,19 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
         CK(cudaMemcpy2D(host_out, 8, ctx->d_r1, 96 * 8, 8, n, cudaMemcpyDeviceToHost));
         return 0;
     }
-    if (what == 9) {
-        if (!ctx->d_tii_res) { ctx->err = "tap 9 needs dabb_options.decode_tii to have been set"; return DABB_E_STATE; }
-        const size_t n = sizeof(dabb_tii_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_tii_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
-    }
-    if (what == 10) {
-        if (!ctx->d_ber_res) { ctx->err = "tap 10 needs dabb_options.count_bit_errors to have been set"; return DABB_E_STATE; }
-        const size_t n = sizeof(dabb_ber_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_ber_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
-    }
-    if (what == 11) {
-        if (!ctx->d_clock_res) { ctx->err = "tap 11 needs dabb_options.sample_clock to have been set"; return DABB_E_STATE; }
-        const size_t n = sizeof(dabb_clock_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_clock_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
-    }
+    if (what == 9) return read_records(ctx, ctx->tii, "tap 9 needs dabb_options.decode_tii to have been set", host_out, bytes);
+    if (what == 10) return read_records(ctx, ctx->ber, "tap 10 needs dabb_options.count_bit_errors to have been set", host_out, bytes);
+    if (what == 11) return read_records(ctx, ctx->clock, "tap 11 needs dabb_options.sample_clock to have been set", host_out, bytes);
+    if (what == 12) return read_records(ctx, ctx->comb, "tap 12 needs dabb_set_combining to have formed a group", host_out, bytes);
     if (what == 13) {
-        if (!ctx->d_acq_res) { ctx->err = "tap 13 needs dabb_options.acquisition to have been set to DABB_ACQ_ROBUST"; return DABB_E_STATE; }
         std::vector<dabb_acq_result> r(ctx->S); std::vector<int32_t> exc(ctx->S);
-        CK(cudaMemcpy(r.data(), ctx->d_acq_res, sizeof(dabb_acq_result) * ctx->S, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(exc.data(), ctx->d_acq_exc, sizeof(int32_t) * ctx->S, cudaMemcpyDeviceToHost));
+        int rc;
+        if ((rc = read_records(ctx, ctx->acq, "tap 13 needs dabb_options.acquisition to have been set to DABB_ACQ_ROBUST", r.data(), sizeof(dabb_acq_result) * ctx->S))) return rc;
+        CK(cudaMemcpy(exc.data(), ctx->acq->exc, sizeof(int32_t) * ctx->S, cudaMemcpyDeviceToHost));
         for (int s = 0; s < ctx->S; s++) r[s].excised = exc[s];
         const size_t n = sizeof(dabb_acq_result) * ctx->S; memcpy(host_out, r.data(), bytes < n ? bytes : n); return 0;
     }
-    if (what == 12) {
-        if (!ctx->d_comb_res) { ctx->err = "tap 12 needs dabb_set_combining to have formed a group"; return DABB_E_STATE; }
-        const size_t n = sizeof(dabb_combine_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_comb_res, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0;
-    }
-    if (what == 4 && ctx->d_tii && ctx->d_null && ctx->decode_tii) { const size_t n = (size_t)ctx->S * 2 * TU * 8; CK(cudaMemcpy(host_out, ctx->d_tii, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
+    if (what == 4 && ctx->d_null && ctx->decode_tii) { const size_t n = (size_t)ctx->S * 2 * TU * 8; CK(cudaMemcpy(host_out, ctx->tii->spectra, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 3 && ctx->d_null) { const size_t n = (size_t)ctx->S * TNULL * 8; CK(cudaMemcpy(host_out, ctx->d_null, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 5) { const size_t n = sizeof(dabb_frame_result) * ctx->S; CK(cudaMemcpy(host_out, ctx->d_results, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
     if (what == 6) { const size_t n = (size_t)ctx->S * 12 * 32; CK(cudaMemcpy(host_out, ctx->d_fibs, bytes < n ? bytes : n, cudaMemcpyDeviceToHost)); return 0; }
@@ -1607,56 +1624,37 @@ int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
         || (opt->soft_demap != DABB_DEMAP_REFERENCE && opt->soft_demap != DABB_DEMAP_WEIGHTED)
         || (opt->sample_clock != DABB_CLOCK_OFF && opt->sample_clock != DABB_CLOCK_TRACK)
         || (opt->acquisition != DABB_ACQ_REFERENCE && opt->acquisition != DABB_ACQ_ROBUST)) return DABB_E_ARG;
-    if (opt->decode_tii && !ctx->d_tii_res) {       // first use of TII: its buffers (64 KB per stream), zeroed = no open combinations
-        cudaSetDevice(ctx->device);
-        sync_all(ctx);
-        const size_t S = (size_t)ctx->S;
-        uint16_t rank[2][dabb_tii::N_ERR];
-        dabb_tii::build_rank_tables(rank);
-        int rc;
-        if ((!ctx->d_null && (rc = dalloc(ctx, ctx->d_tii_null, S * TNULL))) || (rc = dalloc(ctx, ctx->d_tii_hdr, S)) || (rc = dalloc(ctx, ctx->d_tii_jobs, S * dabb_tii::MAX_JOBS)) ||
-            (rc = dalloc(ctx, ctx->d_tii_njobs, S)) || (rc = dalloc(ctx, ctx->d_tii_sums, S * dabb_tii::N_SLOTS * dabb_tii::N_ERR)) || (rc = dalloc(ctx, ctx->d_tii_rank, 2 * dabb_tii::N_ERR))) {
-            ctx->d_tii_null.reset(); ctx->d_tii_hdr.reset(); ctx->d_tii_jobs.reset(); ctx->d_tii_njobs.reset(); ctx->d_tii_sums.reset(); ctx->d_tii_rank.reset();
-            return rc;
-        }
-        CK(cudaMemcpyAsync(ctx->d_tii_rank, rank, sizeof rank, cudaMemcpyHostToDevice, ctx->stream));
-        if ((rc = dalloc(ctx, ctx->d_tii_res, S))) return rc;      // last: it marks the analysis as available
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    if (opt->count_bit_errors && !ctx->d_ber_res) {     // first use of the bit-error count: the puncturing of every profile so far and of the FIC
-        cudaSetDevice(ctx->device);
-        sync_all(ctx);
-        int rc;
-        if ((rc = dalloc(ctx, ctx->d_ber_prof, DABB_MAX_PROFILES + 1))) return rc;
-        for (size_t i = 0; i < ctx->profiles.size(); i++) CK(cudaMemcpyAsync(ctx->d_ber_prof + i, &ctx->profiles[i].ber, sizeof(dabb_ber::Profile), cudaMemcpyHostToDevice, ctx->stream));
-        CK(cudaMemcpyAsync(ctx->d_ber_prof + DABB_MAX_PROFILES, &ctx->h_ber_fic, sizeof(dabb_ber::Profile), cudaMemcpyHostToDevice, ctx->stream));
-        if ((rc = dalloc(ctx, ctx->d_ber_res, (size_t)ctx->S))) { ctx->d_ber_prof.reset(); return rc; }      // last: it marks the count as available
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    if (opt->sample_clock == DABB_CLOCK_TRACK && !ctx->d_clock_res) {     // first use of clock tracking: the per-frame ppm and the records
-        cudaSetDevice(ctx->device);
-        sync_all(ctx);
-        int rc;
-        if ((rc = dalloc(ctx, ctx->d_clock_frame, 2 * (size_t)ctx->S))) return rc;
-        if ((rc = dalloc(ctx, ctx->d_clock_res, (size_t)ctx->S))) { ctx->d_clock_frame.reset(); return rc; }      // last: it marks tracking as available
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    if (opt->acquisition == DABB_ACQ_ROBUST && !ctx->d_acq_res) {     // first use of the robust search: its tables, scratch and records
-        cudaSetDevice(ctx->device);
-        sync_all(ctx);
-        const size_t S = (size_t)ctx->S;
-        float cos_tab[dabb_acq::BLK];
-        dabb_acq::make_cos_table(cos_tab);
-        int rc;
-        if ((rc = dalloc(ctx, ctx->d_acq_cos, dabb_acq::BLK)) || (rc = dalloc(ctx, ctx->d_acq_job, S)) || (rc = dalloc(ctx, ctx->d_acq_level, S * dabb_acq::NB_MAX)) ||
-            (rc = dalloc(ctx, ctx->d_acq_l1, S * dabb_acq::NB_MAX)) || (rc = dalloc(ctx, ctx->d_acq_exc, S))) {
-            ctx->d_acq_cos.reset(); ctx->d_acq_job.reset(); ctx->d_acq_level.reset(); ctx->d_acq_l1.reset(); ctx->d_acq_exc.reset();
-            return rc;
-        }
-        CK(cudaMemcpyAsync(ctx->d_acq_cos, cos_tab, sizeof cos_tab, cudaMemcpyHostToDevice, ctx->stream));
-        if ((rc = dalloc(ctx, ctx->d_acq_res, S))) return rc;      // last: it marks the search as available
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
+    const size_t S = (size_t)ctx->S;
+    int rc;
+    if ((rc = enable(ctx, opt->decode_tii, ctx->tii, [&](Tii& t) -> int {        // zeroed: no open combinations
+            uint16_t rank[2][dabb_tii::N_ERR];
+            dabb_tii::build_rank_tables(rank);
+            if ((!ctx->d_null && (rc = dalloc(ctx, t.null, S * TNULL))) || (rc = dalloc(ctx, t.spectra, S * 2 * TU)) || (rc = dalloc(ctx, t.hdr, S)) ||
+                (rc = dalloc(ctx, t.jobs, S * dabb_tii::MAX_JOBS)) || (rc = dalloc(ctx, t.njobs, S)) || (rc = dalloc(ctx, t.sums, S * dabb_tii::N_SLOTS * dabb_tii::N_ERR)) ||
+                (rc = dalloc(ctx, t.rank, 2 * dabb_tii::N_ERR)) || (rc = dalloc(ctx, t.res, S)))
+                return rc;
+            CK(cudaMemcpyAsync(t.rank, rank, sizeof rank, cudaMemcpyHostToDevice, ctx->stream));
+            return DABB_OK;
+        })) ||
+        (rc = enable(ctx, opt->count_bit_errors, ctx->ber, [&](Ber& b) -> int {        // the puncturing of every profile so far and of the FIC
+            if ((rc = dalloc(ctx, b.prof, DABB_MAX_PROFILES + 1)) || (rc = dalloc(ctx, b.res, S))) return rc;
+            for (size_t i = 0; i < ctx->profiles.size(); i++) CK(cudaMemcpyAsync(b.prof + i, &ctx->profiles[i].ber, sizeof(dabb_ber::Profile), cudaMemcpyHostToDevice, ctx->stream));
+            dabb_ber::Profile fic{}; const int fic_L[2] = {21, 3}, fic_PI[2] = {16, 15};
+            build_ber_profile(*ctx->host, 2, fic_L, fic_PI, 768, fic); fic.prbs = ctx->d_fic_prbs_words;
+            CK(cudaMemcpyAsync(b.prof + DABB_MAX_PROFILES, &fic, sizeof fic, cudaMemcpyHostToDevice, ctx->stream));
+            return DABB_OK;
+        })) ||
+        (rc = enable(ctx, opt->sample_clock == DABB_CLOCK_TRACK, ctx->clock, [&](Clock& c) { return (rc = dalloc(ctx, c.frame, 2 * S)) ? rc : dalloc(ctx, c.res, S); })) ||
+        (rc = enable(ctx, opt->acquisition == DABB_ACQ_ROBUST, ctx->acq, [&](Acq& a) -> int {
+            float cos_tab[dabb_acq::BLK];
+            dabb_acq::make_cos_table(cos_tab);
+            if ((rc = dalloc(ctx, a.cos, dabb_acq::BLK)) || (rc = dalloc(ctx, a.job, S)) || (rc = dalloc(ctx, a.level, S * dabb_acq::NB_MAX)) ||
+                (rc = dalloc(ctx, a.l1, S * dabb_acq::NB_MAX)) || (rc = dalloc(ctx, a.exc, S)) || (rc = dalloc(ctx, a.res, S)))
+                return rc;
+            CK(cudaMemcpyAsync(a.cos, cos_tab, sizeof cos_tab, cudaMemcpyHostToDevice, ctx->stream));
+            return DABB_OK;
+        })))
+        return rc;
     ctx->disable_coarse = opt->disable_coarse != 0; ctx->placement = opt->fft_placement; ctx->freqsync = opt->freqsync_method; ctx->decode_tii = opt->decode_tii != 0;
     ctx->count_ber = opt->count_bit_errors != 0; ctx->soft_demap = opt->soft_demap; ctx->sample_clock = opt->sample_clock;
     ctx->acquisition = opt->acquisition;
