@@ -226,6 +226,44 @@ typedef struct {
     struct { int32_t codewords, bits, errors, erasures; } subch[DABB_MAX_SUBCH];
 } dabb_ber_result;
 
+/* Modulation error ratio (MER) of one stream in one step: tap 14, while dabb_set_mer is on (replaces: none; the reference's only signal
+ * figure is OfdmDecoder::get_snr, dabb_frame_result.snr_raw, measured on bins outside the ensemble's 1536 carriers).
+ * MER is measured on the softbits the FIC decoder reads, so it shows what the decoder is given.  Under DABB_DEMAP_REFERENCE the softbits
+ * of a carrier are trunc(-Re r1 127 / l1) and trunc(-Im r1 127 / l1), l1 = |Re r1| + |Im r1|, which fixes the phase of r1 to within
+ * the 8-bit quantization.  For one carrier with softbits a (Re) and b (Im):
+ *   u = |a| + |b|,  v = |a| - |b|        (int32; a, b the int8 softbits, -128 read as -128)
+ * v / u = tan(pi/4 - theta), theta the angle of r1 folded into its quadrant, so v^2 / u^2 is the squared error of the unit-normalised
+ * product against its nearest DQPSK point and u^2 that point's power.  For a stream whose step has status DABB_FRAME_DECODED, with the
+ * measurement on:
+ *   points: data symbols l = 1, 2, 3 (the FIC's: softbits [l - 1][0 .. 3071] of tap 0, in every decoded frame whatever the symbol mask,
+ *     keep_taps or sub-channel selection), logical carriers i = 0 .. 1535, a = soft[i], b = soft[1536 + i];
+ *   group: logical carrier i is physical carrier k = perm[i] (the frequency interleaver, freq-interleaver.cpp:35-59), k in [-768, 768]
+ *     without 0; its group is g = (k + 768 - (k > 0)) / 24, 0 .. 63 with 24 carriers each, lowest frequency first;
+ *   sig = sum of u^2 and err = sum of v^2 over the 4608 points, exact int64; group[g].sig / .err the same sums over the group's 72
+ *     points, int32 (at most 72 * 256^2 < 2^31); points = the number of the 4608 points with u > 0;
+ *   mer_db = 10 log10(sig / err) in double, rounded to float; +INFINITY when err == 0 < sig, 0 when sig == 0.
+ * Every other stream, and every stream of a step run with the measurement off, gets an all-zero record.  The sums are integers, so a
+ * record depends neither on the batch size, ofdm_groups, the tail split, keep_taps nor the stream index.
+ * The softbits are those the FIC decoder reads: a diversity leader's are the combined ones (the record shows the combination's gain),
+ * its members keep their own antenna's; under DABB_CLOCK_TRACK they are the derotated ones.  Under DABB_DEMAP_WEIGHTED a carrier below
+ * the symbol's geometric-mean level has smaller softbits, so it weighs less in sig / err and its phase is resolved more coarsely:
+ * compare MER only between streams under the same demap.
+ * Meaning (a model of one carrier pair, reference demap, AWGN on both symbols): from 12 to 40 dB per-carrier SNR the MER follows the SNR
+ * within 0.9 dB; below about 10 dB it saturates towards 5.6 dB (the decision-directed floor, where tap 10's bit errors take over); above
+ * about 40 dB the 8-bit softbits cannot resolve the phase.  Valid range: 10 to 40 dB of per-carrier SNR, which is the SNR over 2.048 MHz
+ * plus 1.25 dB (10 log10(2048 / 1536)).  The 64-group profile shows multipath notches, narrowband interferers and band-edge roll-off.
+ * dabb_set_mer(ctx, 1) switches the measurement on, dabb_set_mer(ctx, 0) off, from the next dabb_process / dabb_submit (steps already
+ * enqueued keep what they were enqueued with).  The first enable allocates the group table and the records and waits for outstanding
+ * work; a context that never enables it allocates and launches nothing for it. */
+enum { DABB_MER_GROUPS = 64 };
+typedef struct {
+    int32_t points;             /* points with u > 0 (at most 4608) */
+    float mer_db;               /* 10 log10(sig / err) */
+    int64_t sig, err;           /* sum of u^2, sum of v^2 over the 4608 points */
+    struct { int32_t sig, err; } group[DABB_MER_GROUPS];
+} dabb_mer_result;
+int dabb_set_mer(dabb_ctx* ctx, int32_t enable);
+
 /* Transmitter identification (TIIDecoder, backend/tii-decoder.cpp:236-383) of one stream in one step: tap 9.  Every decoded frame is
  * analysed while dabb_options.decode_tii is set; each (comb, pattern) combination found in a frame accumulates its phase-error table over
  * five analyses and is then reported once, like onTIIMeasurement.  A frame reports at most DABB_TII_MAX combinations (the reference
@@ -390,7 +428,9 @@ int dabb_profile_read(dabb_ctx* ctx, char* json_out, size_t cap);
  *       dabb_options.sample_clock has been set to DABB_CLOCK_TRACK once
  *  12 = dabb_combine_result [n_streams] of the last step (all zero when that step ran without a group); DABB_E_STATE until
  *       dabb_set_combining has formed a group of two or more streams once
- *  13 = dabb_acq_result [n_streams] of the last step; DABB_E_STATE until dabb_options.acquisition has been set to DABB_ACQ_ROBUST once */
+ *  13 = dabb_acq_result [n_streams] of the last step; DABB_E_STATE until dabb_options.acquisition has been set to DABB_ACQ_ROBUST once
+ *  14 = dabb_mer_result [n_streams] of the last step (all zero when that step ran with the measurement off); DABB_E_STATE until
+ *       dabb_set_mer(ctx, 1) has been called once */
 int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes);
 
 /* ---------------------------------------------------------------------------------------------------------

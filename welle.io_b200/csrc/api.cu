@@ -5,6 +5,7 @@
 #include "common.cuh"
 #include "viterbi.cuh"
 #include "survey_core.cuh"
+#include "mer_core.cuh"
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -99,6 +100,8 @@ struct Clock { DevBuf<float> frame; DevBuf<dabb_clock_result> res; };
 // robust acquisition (acq.cu): the cosine table of the block transform, each stream's search span, the block levels and envelope sums
 // [S][NB_MAX], the bins the excising find_index instance zeroed [S] (tap 13's `excised`, merged when it is read)
 struct Acq { DevBuf<float> cos, level, l1; DevBuf<AcqJob> job; DevBuf<int32_t> exc; DevBuf<dabb_acq_result> res; };
+// modulation error ratio (mer.cu): each logical carrier's group [KC]
+struct Mer { DevBuf<uint8_t> group; DevBuf<dabb_mer_result> res; };
 // diversity combining (combine.cu): the tables of one grouping, built whole by rebuild_comb.  Per group its members and their r1 rows
 // (groups) and the (group, symbol) items of combine_kernel; per stream its group or -1 (gid).  Without keep_taps the OFDM kernel stores
 // the grouped streams' r1 of their leader's symbols in r1 (row[s], the symbols lmask[s] marks); with it combine_kernel reads tap 2.
@@ -118,7 +121,8 @@ struct dabb_ctx {
     cudaStream_t stream2 = nullptr; cudaEvent_t ev_ofdm = nullptr, ev_fic = nullptr; DevBuf<uint2> d_dec_fic; int S = 0; int fft_mode = 0; int disable_coarse = 0; int keep_taps = 0; int placement = 0; int freqsync = 0;
     // the optional analyses, null until first enabled, and the options that run them in a step (combining runs while comb->tab exists)
     std::unique_ptr<Tii> tii; std::unique_ptr<Ber> ber; std::unique_ptr<Clock> clock; std::unique_ptr<Acq> acq; std::unique_ptr<Combining> comb;
-    int decode_tii = 0, count_ber = 0, sample_clock = DABB_CLOCK_OFF, acquisition = DABB_ACQ_REFERENCE;
+    std::unique_ptr<Mer> mer;
+    int decode_tii = 0, count_ber = 0, sample_clock = DABB_CLOCK_OFF, acquisition = DABB_ACQ_REFERENCE, measure_mer = 0;
     TraceBuf trace{nullptr, nullptr, 0}; std::string trace_path; int n_slots = 1; int max_cu = 144; int ring_pitch = 0;
     DevBuf<unsigned long long> d_trace_rec; DevBuf<unsigned int> d_trace_count;      // what `trace` points into
     std::string err; int64_t launches = 0; int osc_mismatches = -1; int osc_patched = 0; std::vector<float2> h_osc;
@@ -1319,6 +1323,12 @@ static int enqueue_step(dabb_ctx* ctx, const dabb_io* io, const float2* iq, int6
     cudaStream_t F = serial ? ctx->stream : ctx->stream2;
     if (!serial) { CK(cudaEventRecord(ctx->ev_ofdm, B)); CK(cudaStreamWaitEvent(F, ctx->ev_ofdm, 0)); }
     if ((rc = run_fic(ctx, d_soft, DABB_SOFT_PER_FRAME, d_active, S, ctx->d_fibs, ctx->d_crc, F, ctx->d_dec_fic))) return rc;
+    // the MER of the softbits the FIC decoder has just read, behind the same wait for lane A and before ev_fic, which guards their reuse
+    if (ctx->measure_mer) {
+        MerParams mp{}; mp.soft = d_soft; mp.soft_stride = DABB_SOFT_PER_FRAME; mp.active = d_active; mp.group = ctx->mer->group; mp.res = ctx->mer->res.get(); mp.n_streams = S;
+        launch_mer(mp, F);
+        if ((rc = check_launch(ctx, "mer_kernel"))) return rc;
+    } else if (ctx->mer && (rc = clear_records(ctx, ctx->mer->res, F))) return rc;     // tap 14: nothing measured in this step
     if (!serial) CK(cudaEventRecord(ctx->ev_fic, F));
     const int32_t* h_info[DABB_MAX_SUBCH] = {nullptr, nullptr, nullptr, nullptr};
     for (int k = 0; k < ctx->n_slots; k++) {
@@ -1519,6 +1529,7 @@ int dabb_read_tap(dabb_ctx* ctx, int32_t what, void* host_out, size_t bytes)
     if (what == 10) return read_records(ctx, ctx->ber, "tap 10 needs dabb_options.count_bit_errors to have been set", host_out, bytes);
     if (what == 11) return read_records(ctx, ctx->clock, "tap 11 needs dabb_options.sample_clock to have been set", host_out, bytes);
     if (what == 12) return read_records(ctx, ctx->comb, "tap 12 needs dabb_set_combining to have formed a group", host_out, bytes);
+    if (what == 14) return read_records(ctx, ctx->mer, "tap 14 needs dabb_set_mer to have been called with enable = 1", host_out, bytes);
     if (what == 13) {
         std::vector<dabb_acq_result> r(ctx->S); std::vector<int32_t> exc(ctx->S);
         int rc;
@@ -1658,6 +1669,22 @@ int dabb_set_options(dabb_ctx* ctx, const dabb_options* opt)
     ctx->disable_coarse = opt->disable_coarse != 0; ctx->placement = opt->fft_placement; ctx->freqsync = opt->freqsync_method; ctx->decode_tii = opt->decode_tii != 0;
     ctx->count_ber = opt->count_bit_errors != 0; ctx->soft_demap = opt->soft_demap; ctx->sample_clock = opt->sample_clock;
     ctx->acquisition = opt->acquisition;
+    return DABB_OK;
+}
+
+int dabb_set_mer(dabb_ctx* ctx, int32_t on)
+{
+    if (!ctx) return DABB_E_ARG;
+    int rc;
+    if ((rc = enable(ctx, on != 0, ctx->mer, [&](Mer& m) -> int {        // each logical carrier's group
+            uint8_t g[KC];
+            for (int i = 0; i < KC; i++) g[i] = (uint8_t)dabb_mer::group_of(ctx->host->perm[i]);
+            if ((rc = dalloc(ctx, m.group, KC, false)) || (rc = dalloc(ctx, m.res, (size_t)ctx->S))) return rc;
+            CK(cudaMemcpyAsync(m.group, g, sizeof g, cudaMemcpyHostToDevice, ctx->stream));
+            return DABB_OK;
+        })))
+        return rc;
+    ctx->measure_mer = on != 0;
     return DABB_OK;
 }
 

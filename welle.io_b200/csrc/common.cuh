@@ -116,6 +116,16 @@ struct CombParams {
 };
 void launch_combine(const CombParams& p, cudaStream_t st);
 
+// ---- modulation error ratio (mer.cu, mer_core.cuh) ----
+struct MerParams {
+    const int8_t* soft; int64_t soft_stride;     // the step's softbits (the FIC decoder's input)
+    const int32_t* active;                       // [S] the step decoded a frame
+    const uint8_t* group;                        // [1536] each logical carrier's group (dabb_mer::group_of of its physical carrier)
+    void* res;                                   // [S] dabb_mer_result (tap 14)
+    int n_streams;
+};
+void launch_mer(const MerParams& p, cudaStream_t st);
+
 // ---- TII analysis (tii.cu, tii_core.cuh) ----
 struct TiiParams {
     const float2* spectra;                       // [n][2][T_u] from tii_spectra_kernel: phase reference symbol, null symbol

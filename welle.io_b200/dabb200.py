@@ -91,6 +91,10 @@ assert COMBINE_DTYPE.itemsize == 16
 # dabb_acq_result: one stream's robust null search and phase reference excision of one step (tap 13)
 ACQ_DTYPE = np.dtype([("searched", "<i4"), ("blocks", "<i4"), ("depth_db", "<f4"), ("excised", "<i4"), ("null_end", "<i8")])
 assert ACQ_DTYPE.itemsize == 24
+# dabb_mer_result: one stream's modulation error ratio of one step, over the band and per group of 24 carriers (tap 14)
+MER_GROUPS = 64
+MER_DTYPE = np.dtype([("points", "<i4"), ("mer_db", "<f4"), ("sig", "<i8"), ("err", "<i8"), ("group", [("sig", "<i4"), ("err", "<i4")], (MER_GROUPS,))])
+assert MER_DTYPE.itemsize == 536
 
 
 class IO(C.Structure):
@@ -103,7 +107,7 @@ EXPORTS = ["dabb_create", "dabb_destroy", "dabb_last_error", "dabb_abi_version",
            "dabb_remove_subchannel", "dabb_set_combining", "dabb_process", "dabb_process_async", "dabb_sync", "dabb_join_lanes", "dabb_submit", "dabb_collect", "dabb_cuda_stream", "dabb_kernel_launches",
            "dabb_read_tap", "dabb_profile", "dabb_profile_read", "dabb_ofdm_demod", "dabb_ofdm_demod_ex", "dabb_find_index", "dabb_find_index_ex", "dabb_coarse_estimate", "dabb_viterbi", "dabb_fic_decode", "dabb_msc_decode",
            "dabb_rs_superframes", "dabb_dev_alloc", "dabb_dev_free", "dabb_memcpy_h2d", "dabb_memcpy_d2h",
-           "dabb_chan_create", "dabb_chan_destroy", "dabb_chan_input_range", "dabb_channelize", "dabb_survey", "dabb_survey_candidates"]
+           "dabb_chan_create", "dabb_chan_destroy", "dabb_chan_input_range", "dabb_channelize", "dabb_survey", "dabb_survey_candidates", "dabb_set_mer"]
 
 
 class ChanConfig(C.Structure):
@@ -306,6 +310,11 @@ class Context:
         t = np.ascontiguousarray(leader, np.int32)
         self._ck(self.lib.dabb_set_combining(self.h, _vp(t), C.c_int32(t.size)))
 
+    def set_mer(self, enable=True):
+        """the modulation error ratio of every decoded frame's FIC softbits, over the band and in MER_GROUPS groups of 24 carriers
+        (dabb_set_mer, tap 14), from the next step on"""
+        self._ck(self.lib.dabb_set_mer(self.h, C.c_int32(int(bool(enable)))))
+
     def process(self, iq, stride, buf_start, buf_len, iq_is_host=False, msc_stride=0, sf_stride=0, want=("results", "fibs"), iq_format=0):
         S = self.n_streams
         bs = np.ascontiguousarray(buf_start, np.int64)
@@ -396,7 +405,7 @@ class Context:
         4 TII spectra (PRS, null symbol), 5 frame results, 6 FIBs, 7 logical frames [S, MAX_SUBCH, 4, stride] and 8 superframes
         [S, MAX_SUBCH, stride] of the last step (also after process_async), 9 TII measurements (TII_DTYPE per stream), 10 channel bit
         errors (BER_DTYPE per stream), 11 sample-clock estimates (CLOCK_DTYPE per stream), 12 diversity combinations (COMBINE_DTYPE per
-        stream), 13 robust acquisition (ACQ_DTYPE per stream)"""
+        stream), 13 robust acquisition (ACQ_DTYPE per stream), 14 modulation error ratio (MER_DTYPE per stream)"""
         if what == 7:
             out = np.zeros((self.n_streams, MAX_SUBCH, 4, stride), np.uint8)
         elif what == 8:
@@ -423,6 +432,8 @@ class Context:
             out = np.zeros(self.n_streams, COMBINE_DTYPE)
         elif what == 13:
             out = np.zeros(self.n_streams, ACQ_DTYPE)
+        elif what == 14:
+            out = np.zeros(self.n_streams, MER_DTYPE)
         else:
             out = np.zeros((self.n_streams, TU), np.float32)
         self._ck(self.lib.dabb_read_tap(self.h, what, _vp(out), C.c_size_t(out.nbytes)))

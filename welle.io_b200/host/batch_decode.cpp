@@ -2,7 +2,7 @@
  * batch_decode.cpp — native batch driver over the C ABI: decodes many RAW IQ recordings at once, one stream per file (or per ensemble of a
  * wideband file, --rate), on one GPU.
  *
- *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock]
+ *   batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--mer] [--soft weighted|reference] [--clock]
  *                [--acq robust|reference] [--diversity N] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file1 [file2 ...]
  *
  * What `welle-cli -f FILE -D` does for one recording (welle-cli.cpp:215-235,612-707: dump the FIC, tune to the first audio
@@ -18,6 +18,12 @@
  *
  * --ber: channel bit errors counted on the device (dabb_options.count_bit_errors, tap 10); every decoded frame adds one line
  * "fic_bits fic_errors fic_erasures codewords bits errors erasures" to DIR/<name>.ber, the last four for the service's slot (0).
+ *
+ * --mer: the modulation error ratio of the FIC softbits, measured on the device (dabb_set_mer, tap 14) in the decode context only (not in
+ * the --scan / --offset auto survey and confirmation contexts).  Every decoded frame adds one line "points mer_db sig err" to
+ * DIR/<name>.mer; at the end DIR/<name>.merprof gets one line "first_carrier last_carrier sig err mer_db" per group of 24 carriers
+ * (DABB_MER_GROUPS, lowest frequency first), sig and err summed in int64 over every decoded frame of the run and mer_db = 10 log10(sig /
+ * err) of those sums (inf when err == 0 < sig, 0 when sig == 0).
  *
  * --soft weighted|reference: the OFDM demodulator's soft-decision demap (dabb_options.soft_demap) of every context the driver creates,
  * the --scan / --offset auto survey and confirmation contexts included.  reference (the default) is the reference decoder's demap and
@@ -43,7 +49,7 @@
  *
  * --rate HZ --offset HZ[,HZ...]: every file is a wideband recording at HZ samples/s (any rate dabb_chan_create accepts) and every offset
  * (Hz from the tuned frequency, may be negative) is one stream of the batch, decoded by a channelizer of the same context (dabb_chan_*):
- * outputs go to DIR/<name>@<offset>.{fic,msc,rs} (and .tii / .ber / .clk), in the formats above.  The streams of one file progress
+ * outputs go to DIR/<name>@<offset>.{fic,msc,rs} (and .tii / .ber / .clk / .mer / .merprof), in the formats above.  The streams of one file progress
  * independently (their own position, acquisition and end of file).  Every step channelizes exactly each stream's [pos, pos + need) of its
  * 2.048 Msps axis into that stream's device window and then runs dabb_process on the windows; the channelizer keeps no state, so nothing
  * is shifted on the device, and the host keeps per file only the input span its live streams still need.
@@ -89,6 +95,8 @@ struct Stream {
     std::string path, name; FILE* in = nullptr; FILE* fic = nullptr; FILE* msc = nullptr; FILE* rs = nullptr; FILE* tii = nullptr; FILE* ber = nullptr; FILE* clk = nullptr;
     FILE* div = nullptr;                                          /* --diversity: a group leader's combinations */
     FILE* acq = nullptr;                                          /* --acq robust: the null searches */
+    FILE* mer = nullptr;                                          /* --mer: every decoded frame's MER */
+    std::vector<int64_t> mer_prof;                                /* --mer: [DABB_MER_GROUPS][2] sig, err summed over the run */
     int64_t buf_start = 0, have = 0, pos = 0, acq_need = 0;      /* logical sample indices; `have` samples are buffered from buf_start */
     bool tracking = false, eof = false, done = false;
     std::unique_ptr<dabb_host::FigDb> db{new dabb_host::FigDb()};
@@ -112,6 +120,7 @@ struct Outputs {
     std::vector<dabb_clock_result> cres;        /* tap 11, read after every step when not empty (--clock) */
     std::vector<dabb_combine_result> dres;      /* tap 12, read after every step when not empty (--diversity) */
     std::vector<dabb_acq_result> ares;          /* tap 13, read after every step when not empty (--acq robust) */
+    std::vector<dabb_mer_result> mres;          /* tap 14, read after every step when not empty (--mer) */
 };
 
 /* the receiver position after one step's result r of stream s: 0 = the stream ended, 1 = no frame decoded, 2 = a frame was decoded */
@@ -156,6 +165,11 @@ bool handle_result(dabb_ctx* ctx, Stream& z, int s, const Outputs& o, bool tii, 
     if (z.div) {
         const dabb_combine_result& d = o.dres[(size_t)s];
         fprintf(z.div, "%d %u %.6e\n", d.members, d.mask, d.noise);
+    }
+    if (z.mer) {
+        const dabb_mer_result& m = o.mres[(size_t)s];
+        fprintf(z.mer, "%d %.3f %lld %lld\n", m.points, m.mer_db, (long long)m.sig, (long long)m.err);
+        for (int g = 0; g < DABB_MER_GROUPS; g++) { z.mer_prof[(size_t)g * 2] += m.group[g].sig; z.mer_prof[(size_t)g * 2 + 1] += m.group[g].err; }
     }
     for (int f = 0; f < 12; f++) {
         const uint8_t* fb = o.fibs.data() + ((size_t)s * 12 + (size_t)f) * 32;
@@ -216,6 +230,20 @@ bool confirm_result(dabb_ctx* ctx, Stream& z, int s, const Outputs& o, int64_t T
     return true;
 }
 
+/* --mer: DIR/<name>.merprof, one line "first_carrier last_carrier sig err mer_db" per carrier group of the run's summed tap-14 records */
+bool write_mer_profile(const std::string& path, const std::vector<int64_t>& prof)
+{
+    FILE* f = fopen(path.c_str(), "w");
+    if (!f) return false;
+    for (int g = 0; g < DABB_MER_GROUPS; g++) {
+        const int first = 24 * g - 768 + (g >= DABB_MER_GROUPS / 2 ? 1 : 0);       /* carrier 0 is not used */
+        const long long sig = prof[(size_t)g * 2], err = prof[(size_t)g * 2 + 1];
+        const double db = sig == 0 ? 0.0 : err == 0 ? INFINITY : 10.0 * log10((double)sig / (double)err);
+        fprintf(f, "%d %d %lld %lld %.3f\n", first, first + 23, sig, err, db);
+    }
+    return fclose(f) == 0;
+}
+
 int bytes_per_sample(int fmt) { return fmt == DABB_IQ_CF32 ? 8 : (fmt == DABB_IQ_U8 || fmt == DABB_IQ_S8) ? 2 : 4; }
 
 /* one dabb_process step of every stream's window, and the taps the options ask for */
@@ -231,6 +259,7 @@ bool step(dabb_ctx* ctx, Outputs& o, std::vector<int64_t>& buf_start, const floa
     if (!o.cres.empty() && dabb_read_tap(ctx, 11, o.cres.data(), o.cres.size() * sizeof(dabb_clock_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     if (!o.dres.empty() && dabb_read_tap(ctx, 12, o.dres.data(), o.dres.size() * sizeof(dabb_combine_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     if (!o.ares.empty() && dabb_read_tap(ctx, 13, o.ares.data(), o.ares.size() * sizeof(dabb_acq_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
+    if (!o.mres.empty() && dabb_read_tap(ctx, 14, o.mres.data(), o.mres.size() * sizeof(dabb_mer_result)) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return false; }
     return true;
 }
 
@@ -498,7 +527,7 @@ bool scan(const std::vector<std::string>& files, int64_t rate, int fmt, int devi
 
 int main(int argc, char** argv)
 {
-    int fmt = DABB_IQ_CF32, device = 0, soft = DABB_DEMAP_REFERENCE, clock = DABB_CLOCK_OFF, acq = DABB_ACQ_REFERENCE; bool coarse = false, tii = false, ber = false; std::string out;
+    int fmt = DABB_IQ_CF32, device = 0, soft = DABB_DEMAP_REFERENCE, clock = DABB_CLOCK_OFF, acq = DABB_ACQ_REFERENCE; bool coarse = false, tii = false, ber = false, mer = false; std::string out;
     int64_t rate = 0; std::vector<int64_t> offsets; bool scan_only = false, auto_offsets = false; int diversity = 0; bool diversity_set = false;
     std::vector<std::string> files;
     for (int i = 1; i < argc; i++) {
@@ -513,6 +542,7 @@ int main(int argc, char** argv)
         else if (a == "--coarse") coarse = true;
         else if (a == "--tii") tii = true;
         else if (a == "--ber") ber = true;
+        else if (a == "--mer") mer = true;
         else if (a == "--clock") clock = DABB_CLOCK_TRACK;
         else if (a == "--diversity" && i + 1 < argc) { diversity = atoi(argv[++i]); diversity_set = true; }
         else if (a == "--soft" && i + 1 < argc) {
@@ -540,7 +570,7 @@ int main(int argc, char** argv)
     }
     if (out.empty() || files.empty() || (rate > 0) != ((int)!offsets.empty() + (int)scan_only + (int)auto_offsets == 1)
         || (rate <= 0 && (scan_only || auto_offsets))) {
-        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--soft weighted|reference] [--clock] [--acq robust|reference] [--diversity N] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
+        fprintf(stderr, "usage: batch_decode [--format cf32|u8|s8|s16le|s16be] [--device N] [--coarse] [--tii] [--ber] [--mer] [--soft weighted|reference] [--clock] [--acq robust|reference] [--diversity N] [--rate HZ --offset HZ[,HZ...]|auto] [--rate HZ --scan] --out DIR file...\n");
         return 2;
     }
     if (diversity_set && (rate > 0 || diversity < 1 || diversity > DABB_MAX_BRANCHES || files.size() % (size_t)diversity)) {
@@ -597,6 +627,7 @@ int main(int argc, char** argv)
         for (int s = 0; s < S; s++) leader[(size_t)s] = s - s % diversity;
         if (dabb_set_combining(ctx, leader.data(), S) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
     }
+    if (mer && dabb_set_mer(ctx, 1) != DABB_OK) { fprintf(stderr, "batch_decode: %s\n", dabb_last_error(ctx)); return 1; }
 
     std::vector<Stream> st((size_t)S);
     std::vector<Wide> wf(wide ? files.size() : 0);
@@ -621,7 +652,8 @@ int main(int argc, char** argv)
         const bool leads = diversity > 1 && s % diversity == 0;
         if (leads) z.div = fopen((out + "/" + z.name + ".div").c_str(), "w");
         if (acq == DABB_ACQ_ROBUST) z.acq = fopen((out + "/" + z.name + ".acq").c_str(), "w");
-        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii) || (ber && !z.ber) || (clock && !z.clk) || (leads && !z.div) || (acq == DABB_ACQ_ROBUST && !z.acq)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
+        if (mer) { z.mer = fopen((out + "/" + z.name + ".mer").c_str(), "w"); z.mer_prof.assign(2 * DABB_MER_GROUPS, 0); }
+        if (!z.fic || !z.msc || !z.rs || (tii && !z.tii) || (ber && !z.ber) || (clock && !z.clk) || (leads && !z.div) || (acq == DABB_ACQ_ROBUST && !z.acq) || (mer && !z.mer)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
         z.acq_need = 3 * TF;
     }
     dabb_stream_reset(ctx, 0, S, 0);
@@ -629,7 +661,7 @@ int main(int argc, char** argv)
     Outputs o;
     o.res.resize((size_t)S); o.fibs.resize((size_t)S * 12 * 32); o.msc.resize((size_t)S * DABB_MAX_SUBCH * 4 * 1152); o.sf.resize((size_t)S * DABB_MAX_SUBCH * 5760);
     o.tres.resize(tii ? (size_t)S : 0); o.bres.resize(ber ? (size_t)S : 0); o.cres.resize(clock ? (size_t)S : 0); o.dres.resize(diversity > 1 ? (size_t)S : 0);
-    o.ares.resize(acq == DABB_ACQ_ROBUST ? (size_t)S : 0);
+    o.ares.resize(acq == DABB_ACQ_ROBUST ? (size_t)S : 0); o.mres.resize(mer ? (size_t)S : 0);
     std::vector<int64_t> buf_start((size_t)S);
 
     int active = S;
@@ -688,6 +720,10 @@ int main(int argc, char** argv)
         printf("%s frames=%ld fibs=%ld fib_crc_ok=%ld service=0x%X bitrate=%d logical_frames=%ld\n", z.name.c_str(), z.frames, z.fibs, z.fibs_ok, z.sid, z.bitrate, z.logical);
         if (z.in) fclose(z.in);
         fclose(z.fic); fclose(z.msc); fclose(z.rs); if (z.tii) fclose(z.tii); if (z.ber) fclose(z.ber); if (z.clk) fclose(z.clk); if (z.div) fclose(z.div); if (z.acq) fclose(z.acq);
+        if (z.mer) {
+            fclose(z.mer);
+            if (!write_mer_profile(out + "/" + z.name + ".merprof", z.mer_prof)) { fprintf(stderr, "batch_decode: cannot write into %s\n", out.c_str()); return 1; }
+        }
     }
     dabb_destroy(ctx);
     return 0;
